@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- train-step samples/sec of the DreamVLA hot path (BASELINE.json metric) on N B200s of one node.
+"""bench.py -- train-step samples/sec of the DreamVLA hot path (BASELINE.json metric) on N H100s of one node.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--batch B_per_gpu] [--config calvin|libero]
+                  [--dump-outputs DIR]
 
 Workload (config.workload): BASELINE.json configs[1] -- CALVIN ABC-D train step, bf16, sequence_length 10, all five
 world-knowledge heads (RGB / depth / DINO / SAM / flow) + DiT action head, L = 1290 backbone tokens, per-GPU batch 2
@@ -9,6 +10,8 @@ world-knowledge heads (RGB / depth / DINO / SAM / flow) + DiT action head, L = 1
 A step = forward + 7 losses + backward + gradient all-reduce (N > 1) + global-norm clip + AdamW.
 `value` times steps on device-resident synthetic inputs (CUDA events, barrier + synchronize both sides, max over ranks);
 `e2e` times the same public API call with pinned-host inputs copied H2D and the loss copied D2H inside the timed region.
+`--dump-outputs DIR` writes what the last timed step produced (see dump_outputs) so that two builds can be compared
+output for output: model, weights and batch are seeded, so the inputs are identical from run to run.
 `--impl reference` times the reference's own algorithm on the host CPU cores (oracle port of the reference modules,
 pinned against the unmodified reference by tests/test_oracle_cpu.py) on a bounded sample of the same workload.
 """
@@ -45,7 +48,12 @@ def parse():
     ap.add_argument("--dropout", type=float, default=0.1)
     ap.add_argument("--no-graph", action="store_true", help="launch every kernel from Python instead of replaying CUDA graphs")
     ap.add_argument("--layers", type=int, default=24, help=argparse.SUPPRESS)  # debugging only; bench lines use 24
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's outputs to DIR/<name>.npy (float32)")
+    args = ap.parse_args()
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs writes the outputs of this package's train step; it is not available with --impl " + args.impl)
+    return args
 
 
 CONFIGS = {
@@ -73,7 +81,7 @@ CONFIGS = {
 
 # ----------------------------------------------------------------------------------------------------------------------
 class ClockSampler(threading.Thread):
-    """Samples nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """Samples nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -137,32 +145,22 @@ class ClockSampler(threading.Thread):
                 "samples": len(sm)}
 
 
-def ncu_gemm_traffic():
-    """DRAM bytes per launch of the dominant kernel from the committed `ncu --set full` capture (profiles/r2_ncu_gemm.txt, last
-    entry: M=8200 N=1024 K=4096 bias + residual, tools/prof_gemm.py) next to that launch's algorithmic bytes."""
-    path = os.path.join(ROOT, "profiles", "r2_ncu_gemm.txt")
-    try:
-        rd = wr = None
-        for line in open(path):
-            t = line.split()
-            if line.strip().startswith("DRAM read"):
-                rd = float(t[2]) * {"Mbyte": 1e6, "Gbyte": 1e9, "Kbyte": 1e3, "byte": 1.0}[t[3]]
-            elif line.strip().startswith("DRAM write"):
-                wr = float(t[2]) * {"Mbyte": 1e6, "Gbyte": 1e9, "Kbyte": 1e3, "byte": 1.0}[t[3]]
-        M, N, K = 8200, 1024, 4096
-        algo = 2 * (M * K + N * K + 2 * M * N) + 2 * N            # A, B, residual in, out; bias
-        return {"traffic": rd + wr, "traffic_algorithmic_bytes": algo, "traffic_launch": f"gemm M={M} N={N} K={K} bias+residual",
-                "traffic_source": "profiles/r2_ncu_gemm.txt (dram__bytes_read.sum + dram__bytes_write.sum)"}
-    except Exception:  # noqa: BLE001
-        return {"traffic": None}
+# Dense BF16 tensor-core rate of the H100 SXM from NVIDIA's data sheet (700 W part): the denominator of the "frac" fields,
+# not a rate this code has reached.
+H100_BF16_DENSE_TFLOPS = 989.0
+PEAK_SOURCE = "NVIDIA H100 SXM data sheet, dense BF16 (not measured)"
 
 
-def measured_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1442.1), "measured (MEASURED_PEAKS.json bf16_tflops_sustained)"
-    return 1400.0, "fallback (B200_PROFILING.md sustained)"
+def dump_outputs(out_dir, loss, params):
+    """What a caller of the timed train step receives from its last step: the loss it returns, and the model it updates in
+    place -- as a fixed, seeded sample of 4 Mi elements of the flat bf16 parameter buffer (16 MB as float32; the whole buffer
+    is ~1.3 GB).  Written as float32 .npy files."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), loss.detach().float().reshape(1).cpu().numpy())
+    n = params.numel()
+    idx = torch.randint(0, n, (min(n, 4 << 20),), generator=torch.Generator().manual_seed(0)).sort().values
+    np.save(os.path.join(out_dir, "params_sample.npy"), params.detach()[idx.to(params.device)].float().cpu().numpy())
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -271,6 +269,8 @@ def run_ours(args):
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     ms = float(t)
     stage("timed region done")
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, loss, eager_step.flat.P)
     ms_per_step = ms / args.steps
     value = B * world / (ms_per_step / 1e3)
     final_loss = float(loss)
@@ -405,7 +405,7 @@ def run_ours(args):
                     print(f"[e2e probe] world={world} {name:18s} {tms:8.3f} ms/step", file=sys.stderr, flush=True)
 
     stage("e2e done")
-    # ---- roofline of the dominant kernel (tcgen05 GEMM) ----------------------------------------------------------------
+    # ---- roofline of the dominant kernel (wgmma GEMM) ------------------------------------------------------------------
     # one eager fwd+bwd records every dvla_gemm launch (shape, layout, epilogue); each distinct launch is then re-issued
     # 5x back to back on the current stream between two CUDA events (no host gaps), and
     #   achieved = sum(count * 2MNK) / sum(count * avg duration)
@@ -458,11 +458,11 @@ def run_ours(args):
                 print(f"[gemm] M={M:6d} N={N:5d} K={K:5d} a_mn={int(a_mn)} b_mn={int(b_mn)} bias={int(hb)} act={act} res={int(hr)} "
                       f"aux={int(ha)} drop={int(hd)} n={cnt:4d} {per*1e3:8.1f} us {2.0*M*N*K/per/1e9:7.0f} TF/s total {cnt*per:7.3f} ms",
                       file=sys.stderr, flush=True)
-        peak, how = measured_peaks()
+        peak = H100_BF16_DENSE_TFLOPS
         ach = fl / (tm * 1e-3) / 1e12 if tm > 0 else 0.0
-        roof = {"bound": "tensor", "kernel": "gemm_tcgen05_kernel (every tcgen05 GEMM launch of one fwd+bwd)",
+        roof = {"bound": "tensor", "kernel": "gemm_wgmma_kernel (every tensor-core GEMM launch of one fwd+bwd)",
                 "achieved": round(ach, 1), "peak": peak, "unit": "TFLOP/s", "frac": round(ach / peak, 4),
-                "peak_source": how, **ncu_gemm_traffic(), "launches": n_tc, "distinct_launch_shapes": len(calls),
+                "peak_source": PEAK_SOURCE, "launches": n_tc, "distinct_launch_shapes": len(calls),
                 "gemm_ms_per_step": round(tm, 3), "gemm_share_of_step": round(tm / ms_per_step, 3),
                 "gemm_tflop_per_step": round(fl / 1e12, 3),
                 "step_model_tflops": round(cfg["tf_per_sample"] * B / (ms_per_step * 1e-3), 1),
@@ -506,11 +506,11 @@ def run_ours(args):
         line = {
             "metric": "train_step_samples_per_sec", "value": round(value, 3), "unit": "samples/s", "n_gpus": world,
             "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": round(ms_per_step, 3),
-            "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
+            "gpu": torch.cuda.get_device_name(dev), "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
             "config": {"workload": cfg["name"], "per_gpu_batch": B, "global_batch": B * world,
                        "seq_len": cfg["model"]["sequence_length"], "parallelism": f"dp{world}",
                        "dropout": args.dropout, "layers": args.layers, "cuda_graph": graphed,
-                       "l2": "inputs+weights+activations per step >> 126 MB L2 (1.3 GB of bf16 weights re-read every step); no explicit flush",
+                       "l2": "inputs+weights+activations per step >> 50 MB L2 (1.3 GB of bf16 weights re-read every step); no explicit flush",
                        "trainable_params": workload_params, "final_loss": final_loss},
             "clocks": sampler.summary() if sampler else None,
             "e2e": e2e, "gpu_launches": int(launches), "roofline": roof, "cpu_baseline": cpu, "extras": extras,
@@ -547,7 +547,7 @@ def quick_train_measure(config, B, dev, dropout=0.1, steps=10, warmup=3):
     e1.record()
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / steps
-    peak, _ = measured_peaks()
+    peak = H100_BF16_DENSE_TFLOPS
     out = {"workload": cfg["name"], "per_gpu_batch": B, "ms_per_step": round(ms, 3), "value": round(B / ms * 1e3, 2),
            "unit": "samples/s", "steps": steps, "step_frac_of_peak": round(cfg["tf_per_sample"] * B / (ms * 1e-3) / peak, 4),
            "final_loss": float(loss)}
@@ -588,8 +588,8 @@ def latency_measure(dev, steps):
 # the reference's algorithm on the GPU, the way the reference runs it: torch eager kernels + cuBLAS + SDPA with the dense
 # additive mask, bf16 (`--precision bf16` casts the model, train.py:122-123), DistributedDataParallel(find_unused_parameters
 # =True) (train.py:173), clip_grad_norm_(0.1) + torch.optim.AdamW every step (train_utils.py:599-608).  The modules are the
-# oracle's functional restatement (pinned to the unmodified reference by tests/test_oracle_cpu.py): /root/reference does not
-# exist on the GPU box.
+# oracle's functional restatement (pinned to the unmodified reference by tests/test_oracle_cpu.py), so that this arm needs
+# nothing outside the repository.
 # ----------------------------------------------------------------------------------------------------------------------
 def reference_gpu_measure(config, B, dev, steps=5, warmup=3, world=1):
     import torch.nn.functional as F
@@ -760,7 +760,7 @@ def cpu_baseline(args, steps=1, warm=0, budget_s=150.0):
         dt = time.perf_counter() - t0
         if i >= warm:
             times.append(dt)
-        if time.perf_counter() - t_all > budget_s and len(times) >= 1:
+        if budget_s is not None and time.perf_counter() - t_all > budget_s and len(times) >= 1:
             break
     sec = sum(times) / len(times)
     return {"value": round(1.0 / sec, 5), "unit": "samples/s", "cores": cores, "kind": "port",
@@ -773,7 +773,7 @@ def run_reference(args):
     if rank != 0:
         return
     cfg = CONFIGS[args.config]
-    cb = cpu_baseline(args, steps=args.steps, warm=min(args.warmup, 1), budget_s=180.0)
+    cb = cpu_baseline(args, steps=args.steps, warm=min(args.warmup, 1), budget_s=None)   # --steps timed steps, however long
     line = {"impl": "reference", "metric": "train_step_samples_per_sec", "value": cb["value"], "unit": "samples/s",
             "n_gpus": args.gpus, "steps": cb["steps_timed"], "warmup": min(args.warmup, 1),
             "ms_per_step": round(cb["s_per_step"] * 1e3, 1), "higher_is_better": True, "scaling": "weak",

@@ -1,4 +1,4 @@
-"""ctypes binding of libdvla_sm100.so (include/dvla.h).  This is the only place Python touches the C ABI.
+"""ctypes binding of libdvla_sm90.so (include/dvla.h).  This is the only place Python touches the C ABI.
 
 The product path has NO fallback: if the shared library is missing or a call fails, a RuntimeError is raised.
 PyTorch is used for device memory and streams only (tensor.data_ptr(), torch.cuda.current_stream()).
@@ -12,7 +12,7 @@ import os
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(_HERE, "lib", "libdvla_sm100.so")
+LIB_PATH = os.path.join(_HERE, "lib", "libdvla_sm90.so")
 
 ACT_NONE, ACT_GELU_ERF, ACT_GELU_TANH, ACT_QUICK_GELU, ACT_RELU, ACT_SILU = range(6)
 ACT_IDS = {None: 0, "none": 0, "gelu": 1, "gelu_erf": 1, "gelu_tanh": 2, "gelu_new": 2, "quick_gelu": 3, "relu": 4,
@@ -104,7 +104,7 @@ def load() -> C.CDLL:
         return _lib
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
-            f"{LIB_PATH} not found: build it with `python -m dreamvla_b200.build` (nvcc, sm_100a). "
+            f"{LIB_PATH} not found: build it with `python -m dreamvla_b200.build` (nvcc, sm_90a). "
             "dreamvla_b200 has no CPU or PyTorch fallback for its kernels.")
     lib = C.CDLL(LIB_PATH)
     lib.dvla_last_error.restype = C.c_char_p
@@ -261,7 +261,7 @@ def attn_fwd(q, k, v, scale, mask_bits=None, tile_flags=None, dropout_p=0.0, dro
 
 
 def attn_bwd(q, k, v, o, d_o, lse, scale, dq, dk, dv, mask_bits=None, tile_flags=None, dropout_p=0.0, dropout_seed=0,
-             dropout_seed_ptr=None, mask_bits_t=None, key_bias=None):
+             dropout_seed_ptr=None, key_bias=None):
     B, Lq, H, _ = q.shape
     Lk = k.shape[1]
     ws = int(load().dvla_attn_bwd_workspace_bytes(_i64(B), _i64(H), _i64(Lq)))
@@ -283,8 +283,6 @@ def attn_bwd(q, k, v, o, d_o, lse, scale, dq, dk, dv, mask_bits=None, tile_flags
     a.mask_words = 0 if mask_bits is None else mask_bits.shape[1]
     a.scale, a.dropout_p, a.dropout_seed = float(scale), float(dropout_p), int(dropout_seed)
     a.dropout_seed_ptr = _ptr(dropout_seed_ptr)
-    a.mask_t = _ptr(mask_bits_t)
-    a.mask_t_words = 0 if mask_bits_t is None else mask_bits_t.shape[1]
     a.key_bias = _ptr(key_bias)
     _check(load().dvla_attn_bwd(C.byref(a), _stream()), "dvla_attn_bwd")
 

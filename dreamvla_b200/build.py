@@ -1,7 +1,7 @@
-"""Builds libdvla_sm100.so (hand-written CUDA for sm_100a) in-tree with nvcc.
+"""Builds libdvla_sm90.so (hand-written CUDA for sm_90a, NVIDIA H100) in-tree with nvcc.
 
-`python -m dreamvla_b200.build` or `__graft_entry__.build()`.  The .so lands in dreamvla_b200/lib/ so that it
-travels with the repo snapshot to the GPU box (built artefacts are git-ignored, not gpurun-ignored).
+`python -m dreamvla_b200.build` or `__graft_entry__.build()`.  The .so lands in dreamvla_b200/lib/ (git-ignored), where
+dreamvla_b200/_lib.py loads it from; nothing is compiled at run time.
 """
 from __future__ import annotations
 
@@ -13,10 +13,10 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
-LIB = os.path.join(LIBDIR, "libdvla_sm100.so")
-SOURCES = ["gemm_sm100.cu", "attention.cu", "attention_small.cu", "attention_fwd_ws.cu", "attention_bwd_ws.cu", "norm_act.cu", "loss_optim.cu", "dit_sampler.cu", "augment.cu", "capi.cu"]
+LIB = os.path.join(LIBDIR, "libdvla_sm90.so")
+SOURCES = ["gemm_sm90.cu", "attention.cu", "attention_small.cu", "norm_act.cu", "loss_optim.cu", "dit_sampler.cu", "augment.cu", "capi.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
 ]
 
@@ -52,7 +52,7 @@ def build_library(force: bool = False, verbose: bool = True) -> str:
     with ThreadPoolExecutor(max_workers=len(SOURCES)) as ex:
         objs = list(ex.map(compile_one, SOURCES))
     tmp = LIB + ".tmp"          # link beside the target, then rename: a reader never sees a half-written library
-    cmd = [nvcc, "-shared", "-o", tmp, *objs, "-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [nvcc, "-shared", "-o", tmp, *objs, "-gencode", "arch=compute_90a,code=sm_90a"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -1,9 +1,9 @@
 // Flash-style multi-head attention for head_dim = 64 with a bit-matrix visibility mask and tile skipping.
 //
-// Data path of THIS file: cp.async -> XOR-swizzled smem tiles -> ldmatrix -> mma.sync.m16n8k16 (bf16, fp32 accumulate),
-// online softmax in registers, no [Lq,Lk] tensor in HBM.  These kernels serve the short sequences of the path (DiT: 4
-// tokens, resampler: 16 queries) and strides a tensor map cannot express; sequences of >= 96 tokens go to the
-// warp-specialised tcgen05 / TMEM kernels of attention_fwd_ws.cu / attention_bwd_ws.cu through the dispatchers below.
+// Data path of the mma.sync kernels: cp.async -> XOR-swizzled smem tiles -> ldmatrix -> mma.sync.m16n8k16 (bf16, fp32 accumulate),
+// online softmax in registers, no [Lq,Lk] tensor in HBM.  These serve short query blocks and strides a tensor map cannot
+// express; long sequences (>= 96) run on the TMA + wgmma warp-specialised kernels further down (attn_fwd_wgmma_kernel,
+// attn_bwd_wgmma_kernel), the short unmasked ones of the DiT on attention_small.cu.
 //
 // Kernels:
 //   attn_fwd_kernel     grid (ceil(Lq/64), H, B), 4 warps x 16 query rows, K/V tiles of 64 keys double-buffered
@@ -13,6 +13,8 @@
 // Masking: tile_flags[qt, kt] in {0 skip, 1 partial, 2 full}; partial tiles test bits of mask[i, j/32].
 #include <stdlib.h>
 #include <string.h>
+
+#include <mutex>
 
 #include "common.cuh"
 #include "../../include/dvla.h"
@@ -33,7 +35,7 @@ struct AttnParams {
   const uint32_t* mask;
   const uint8_t* tile_flags;
   int B, H, Lq, Lk, nqt, nkt, mask_words;
-  int qt0, kt0;          // first q / kv 64-row tile of this launch (tail launches next to the tcgen05 kernels)
+  int qt0, kt0;          // first q / kv 64-row tile of this launch
   long long q_sb, q_ss, q_sh, k_sb, k_ss, k_sh, v_sb, v_ss, v_sh, o_sb, o_ss, o_sh;
   long long do_sb, do_ss, do_sh, dq_sb, dq_ss, dq_sh, dk_sb, dk_ss, dk_sh, dv_sb, dv_ss, dv_sh;
   float scale;
@@ -317,6 +319,203 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnParams p) {
   }
 }
 
+// ============================================= forward, wgmma + TMA ===============================================
+// Warp-specialised forward for sequences of >= 96 queries.  CTA = 288 threads over the q-tiles 2x and 2x+1 (64 queries
+// each) of one (b, h):
+//   warps 0-3 / 4-7  consumer warpgroup g: S = Q_g K^T (wgmma m64n64k16, both operands from smem), mask / online softmax /
+//                    dropout in registers (the per-warp accumulator layout equals mma.sync's C fragment, so the code below
+//                    is that of attn_fwd_kernel), P -> bf16 register A operand, O += P V (wgmma, V read MN-major)
+//   warp 8           TMA producer (one thread): Q of both tiles once, then K/V tiles of 64 keys through a 3-stage ring
+//                    (mbarrier tx); a K/V tile is loaded when either q-tile sees part of it, and both groups release it.
+// 4-D tensor maps (d, seq|head, head|seq, batch) address q/k/v in place in the fused QKV buffer; rows past L are zero.
+constexpr int WF_STAGES = 3;
+constexpr int WF_THREADS = 288;
+constexpr int WF_SMEM = 1024 + 2 * 8192 + WF_STAGES * 2 * 8192 + 128;
+
+__device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2, int c3) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
+      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      : "memory");
+}
+// 64 rows [row0, row0 + 64) of head h, batch b
+__device__ __forceinline__ void tma_rows(uint32_t dst, const CUtensorMap* m, uint64_t* bar, int head_inner, int row0, int h, int b) {
+  if (head_inner) tma_load_4d(dst, m, bar, 0, h, row0, b);
+  else            tma_load_4d(dst, m, bar, 0, row0, h, b);
+}
+
+struct WgmmaFwdMaps { CUtensorMap q, k, v; int q_head_inner, k_head_inner, v_head_inner; };
+
+__global__ void __launch_bounds__(WF_THREADS, 2) attn_fwd_wgmma_kernel(const __grid_constant__ WgmmaFwdMaps tm, const AttnParams p) {
+  extern __shared__ uint8_t wf_smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(wf_smem_raw) + 1023) & ~uintptr_t(1023));
+  const uint32_t sQ = smem_u32(smem);                       // [2][64 x 128 B]
+  const uint32_t sKV = sQ + 2 * 8192;                       // [stage][K 8 KB | V 8 KB]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 2 * 8192 + WF_STAGES * 2 * 8192);
+  uint64_t* q_full = bars;
+  uint64_t* full = bars + 1;
+  uint64_t* empty = full + WF_STAGES;
+  const int h = blockIdx.x, b = blockIdx.y;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  // late query blocks see the most keys under block-causal masks; blockIdx.z is the slowest launch dimension, so every
+  // (b, h) starts its heavy blocks before any light one
+  const int qt_base = 2 * (static_cast<int>(gridDim.z) - 1 - static_cast<int>(blockIdx.z));
+  const uint8_t* fl0 = p.tile_flags ? p.tile_flags + static_cast<long long>(qt_base) * p.nkt : nullptr;
+  const bool has1 = qt_base + 1 < p.nqt;
+  auto needed = [&](int kt, int g) -> bool {   // does q-tile qt_base+g see any key of k-tile kt?
+    if (g == 1 && !has1) return false;
+    return !fl0 || fl0[g * p.nkt + kt] != 0;
+  };
+  auto next_tile = [&](int kt) {
+    while (kt < p.nkt && !needed(kt, 0) && !needed(kt, 1)) ++kt;
+    return kt;
+  };
+
+  if (threadIdx.x == 0) {
+    mbar_init(q_full, 1);
+    for (int st = 0; st < WF_STAGES; ++st) { mbar_init(&full[st], 1); mbar_init(&empty[st], 8); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp == 8) {
+    // ------------------------------------------------ TMA producer ------------------------------------------------
+    if (lane == 0) {
+      tma_prefetch_desc(&tm.q); tma_prefetch_desc(&tm.k); tma_prefetch_desc(&tm.v);
+      mbar_expect_tx(q_full, 2 * 8192);
+      tma_rows(sQ, &tm.q, q_full, tm.q_head_inner, qt_base * 64, h, b);
+      tma_rows(sQ + 8192, &tm.q, q_full, tm.q_head_inner, qt_base * 64 + 64, h, b);   // past Lq: zero rows
+      int st = 0; uint32_t ph = 0;
+      for (int kt = next_tile(0); kt < p.nkt; kt = next_tile(kt + 1)) {
+        mbar_wait<false>(&empty[st], ph ^ 1);
+        mbar_expect_tx(&full[st], 2 * 8192);
+        tma_rows(sKV + st * 16384, &tm.k, &full[st], tm.k_head_inner, kt * 64, h, b);
+        tma_rows(sKV + st * 16384 + 8192, &tm.v, &full[st], tm.v_head_inner, kt * 64, h, b);
+        if (++st == WF_STAGES) { st = 0; ph ^= 1; }
+      }
+    }
+    return;
+  }
+
+  // -------------------------------------------------- consumers ---------------------------------------------------
+  const int g = warp >> 2, wq = warp & 3;         // consumer group (q-tile qt_base + g), warp within the group
+  const int qt = qt_base + g, q0 = qt * 64;
+  const int c = lane & 3, gr = lane >> 2;
+  const uint8_t* flags = fl0 ? fl0 + g * p.nkt : nullptr;
+  const long long bh = static_cast<long long>(b) * p.H + h;
+  const float sc = p.scale * LOG2E;
+  float o[8][4];
+  zero_c(o);
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  mbar_wait<false>(q_full, 0);
+  const uint32_t qa = sQ + g * 8192;
+
+  int st = 0; uint32_t ph = 0;
+  for (int kt = next_tile(0); kt < p.nkt; kt = next_tile(kt + 1)) {
+    mbar_wait<false>(&full[st], ph);
+    const int flag = flags ? flags[kt] : 2;
+    if (flag != 0 && (g == 0 || has1)) {
+      const uint32_t ka = sKV + st * 16384, va = ka + 8192;
+      float s[8][4];
+      float (&sd)[32] = *reinterpret_cast<float(*)[32]>(&s[0][0]);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_m64n64k16_ss(sd, make_smem_desc_sw128(qa + k * 32, 16, 1024), make_smem_desc_sw128(ka + k * 32, 16, 1024), k != 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_operand32(sd);
+
+      // ---- mask + scale (log2 domain), as attn_fwd_kernel ----
+      const int k0 = kt * 64;
+      const bool tail = (k0 + 64 > p.Lk);
+      uint32_t w[2][2] = {{0xffffffffu, 0xffffffffu}, {0xffffffffu, 0xffffffffu}};
+      if (flag == 1) {
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const int row = q0 + wq * 16 + gr + r * 8;
+#pragma unroll
+          for (int ww = 0; ww < 2; ++ww) {
+            const int wi = kt * 2 + ww;
+            w[r][ww] = (row < p.Lq && wi < p.mask_words) ? p.mask[static_cast<long long>(row) * p.mask_words + wi] : 0u;
+          }
+        }
+      }
+      float tmax[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+      for (int t = 0; t < 8; ++t) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int r = e >> 1;
+          const int kk = t * 8 + 2 * c + (e & 1);
+          bool vis = true;
+          if (flag == 1) vis = (w[r][kk >> 5] >> (kk & 31)) & 1u;
+          if (tail) vis = vis && (k0 + kk < p.Lk);
+          const float v = vis ? s[t][e] * sc : -INFINITY;
+          s[t][e] = v;
+          tmax[r] = fmaxf(tmax[r], v);
+        }
+      }
+      float alpha[2], muse[2];
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const float mn = fmaxf(m_run[r], quad_max(tmax[r]));
+        muse[r] = (mn == -INFINITY) ? 0.f : mn;
+        alpha[r] = exp2f(m_run[r] - muse[r]);
+        m_run[r] = mn;
+        l_run[r] *= alpha[r];
+      }
+#pragma unroll
+      for (int t = 0; t < 8; ++t) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int r = e >> 1;
+          const float pv = exp2f(s[t][e] - muse[r]);
+          s[t][e] = pv;
+          l_run[r] += pv;
+          o[t][e] *= alpha[r];
+        }
+      }
+      if (p.drop_scale != 0.f) {
+        uint32_t keep[8];
+        dropout_bits(p, bh, q0 + wq * 16, k0, false, keep);
+#pragma unroll
+        for (int t = 0; t < 8; ++t)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) s[t][e] = ((keep[t] >> e) & 1u) ? s[t][e] * p.drop_scale : 0.f;
+      }
+      uint32_t pa[4][4];
+      c_to_a(s, pa);
+      float (&od)[32] = *reinterpret_cast<float(*)[32]>(&o[0][0]);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) wgmma_m64n64k16_rs_tb(od, pa[kk], make_smem_desc_sw128(va + kk * 2048, 8192, 1024));
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_operand32(od);
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[st]);
+    if (++st == WF_STAGES) { st = 0; ph ^= 1; }
+  }
+  if (g == 1 && !has1) return;
+
+  // ---- finalize, as attn_fwd_kernel ----
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const float l = quad_sum(l_run[r]);
+    const float inv = l > 0.f ? 1.0f / l : 0.f;
+    const int row = q0 + wq * 16 + gr + r * 8;
+    if (row < p.Lq) {
+      bf16* dst = p.out + b * p.o_sb + static_cast<long long>(row) * p.o_ss + h * p.o_sh;
+#pragma unroll
+      for (int t = 0; t < 8; ++t)
+        *reinterpret_cast<uint32_t*>(dst + t * 8 + 2 * c) = pack_bf16x2(o[t][2 * r] * inv, o[t][2 * r + 1] * inv);
+      if (p.lse && c == 0) p.lse[(bh * p.Lq) + row] = (l > 0.f) ? (m_run[r] + log2f(l)) * LN2 : -INFINITY;
+    }
+  }
+}
+
 // ===================================================== delta ======================================================
 __global__ void __launch_bounds__(256) attn_delta_kernel(const AttnParams p) {
   // 8 lanes per (b, h, i) row of 64 elements
@@ -545,6 +744,234 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const AttnParams p) {
   }
 }
 
+// ============================================ backward, wgmma + TMA ================================================
+// Warp-specialised backward for sequences of >= 96 on both sides, in the S^T / dP^T formulation of attn_bwd_dkv_kernel and
+// the S / dP one of attn_bwd_dq_kernel (same masking, LSE recompute and dropout regeneration):
+//   DKV = true : CTA = key tiles 2x, 2x+1 of one (b, h); consumer group g owns key tile 2x+g (K, V loaded once) and streams
+//                query tiles (Q, dO): S^T = K Q^T, dP^T = V dO^T (wgmma, smem x smem), dV += P^T dO, dK += dS^T Q (wgmma,
+//                register A operand, Q / dO read MN-major)
+//   DKV = false: CTA = query tiles 2x, 2x+1; group g owns query tile 2x+g (Q, dO) and streams key tiles (K, V):
+//                S = Q K^T, dP = dO V^T, dQ += dS K
+// Warp 8 is the TMA producer (3-stage ring of streamed tile pairs); a streamed tile is loaded when either group sees it.
+struct WgmmaBwdMaps { CUtensorMap f0, f1, s0, s1; int f0_hi, f1_hi, s0_hi, s1_hi; };
+
+template <bool DKV>
+// One CTA per SM: dK and dV accumulators next to S and dP need ~160 registers (two CTAs of 9 warps cap a thread at 96).
+__global__ void __launch_bounds__(WF_THREADS, 1) attn_bwd_wgmma_kernel(const __grid_constant__ WgmmaBwdMaps tm, const AttnParams p) {
+  extern __shared__ uint8_t wb_smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(wb_smem_raw) + 1023) & ~uintptr_t(1023));
+  const uint32_t sF = smem_u32(smem);                       // [group][f0 8 KB | f1 8 KB]
+  const uint32_t sS = sF + 4 * 8192;                        // [stage][s0 8 KB | s1 8 KB]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 4 * 8192 + WF_STAGES * 2 * 8192);
+  uint64_t* f_full = bars;
+  uint64_t* full = bars + 1;
+  uint64_t* empty = full + WF_STAGES;
+  const int h = blockIdx.x, b = blockIdx.y;
+  const int nf = DKV ? p.nkt : p.nqt;                       // tiles on the fixed side
+  const int ns = DKV ? p.nqt : p.nkt;                       // tiles on the streamed side
+  const int nfb = (nf + 1) / 2;
+  // heaviest blocks first under block-causal masks: early key tiles are seen by the most queries, late query tiles see
+  // the most keys; blockIdx.z is the slowest launch dimension, so every (b, h) starts its heavy blocks before any light one
+  const int ft_base = 2 * (DKV ? static_cast<int>(blockIdx.z) : nfb - 1 - static_cast<int>(blockIdx.z));
+  const bool has1 = ft_base + 1 < nf;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  auto flag_of = [&](int st_, int g) -> int {               // tile flag of (fixed tile ft_base+g, streamed tile st_)
+    if (g == 1 && !has1) return 0;
+    if (!p.tile_flags) return 2;
+    const int ft = ft_base + g;
+    return DKV ? p.tile_flags[static_cast<long long>(st_) * p.nkt + ft] : p.tile_flags[static_cast<long long>(ft) * p.nkt + st_];
+  };
+  auto next_tile = [&](int t) {
+    while (t < ns && flag_of(t, 0) == 0 && flag_of(t, 1) == 0) ++t;
+    return t;
+  };
+
+  if (threadIdx.x == 0) {
+    mbar_init(f_full, 1);
+    for (int st = 0; st < WF_STAGES; ++st) { mbar_init(&full[st], 1); mbar_init(&empty[st], 8); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp == 8) {
+    if (lane == 0) {
+      tma_prefetch_desc(&tm.f0); tma_prefetch_desc(&tm.f1); tma_prefetch_desc(&tm.s0); tma_prefetch_desc(&tm.s1);
+      mbar_expect_tx(f_full, 4 * 8192);
+      for (int g = 0; g < 2; ++g) {                         // a tile past the sequence end is zero-filled
+        tma_rows(sF + g * 16384, &tm.f0, f_full, tm.f0_hi, (ft_base + g) * 64, h, b);
+        tma_rows(sF + g * 16384 + 8192, &tm.f1, f_full, tm.f1_hi, (ft_base + g) * 64, h, b);
+      }
+      int st = 0; uint32_t ph = 0;
+      for (int t = next_tile(0); t < ns; t = next_tile(t + 1)) {
+        mbar_wait<false>(&empty[st], ph ^ 1);
+        mbar_expect_tx(&full[st], 2 * 8192);
+        tma_rows(sS + st * 16384, &tm.s0, &full[st], tm.s0_hi, t * 64, h, b);
+        tma_rows(sS + st * 16384 + 8192, &tm.s1, &full[st], tm.s1_hi, t * 64, h, b);
+        if (++st == WF_STAGES) { st = 0; ph ^= 1; }
+      }
+    }
+    return;
+  }
+
+  const int g = warp >> 2, wq = warp & 3;
+  const int c = lane & 3, gr = lane >> 2;
+  const int f0 = (ft_base + g) * 64;                        // first key (DKV) / query (dQ) row of this group
+  const long long bh = static_cast<long long>(b) * p.H + h;
+  const float sc = p.scale * LOG2E;
+  const uint32_t fa0 = sF + g * 16384, fa1 = fa0 + 8192;   // DKV: K, V of the key tile; dQ: Q, dO of the query tile
+  float acc0[8][4], acc1[8][4];                             // DKV: dK, dV; dQ: dQ (acc1 unused)
+  zero_c(acc0);
+  zero_c(acc1);
+  float lse2[2], dlt[2];
+  if (!DKV) {
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int row = f0 + wq * 16 + gr + r * 8;
+      lse2[r] = (row < p.Lq) ? p.lse[bh * p.Lq + row] * LOG2E : INFINITY;
+      dlt[r] = (row < p.Lq) ? p.delta[bh * p.Lq + row] : 0.f;
+    }
+  }
+  mbar_wait<false>(f_full, 0);
+
+  int st = 0; uint32_t ph = 0;
+  for (int t = next_tile(0); t < ns; t = next_tile(t + 1)) {
+    mbar_wait<false>(&full[st], ph);
+    const int flag = flag_of(t, g);
+    if (flag != 0) {
+      const uint32_t sa0 = sS + st * 16384, sa1 = sa0 + 8192;   // DKV: Q, dO of the query tile; dQ: K, V of the key tile
+      const int s0r = t * 64;
+      float s[8][4], dp[8][4];
+      float (&sd)[32] = *reinterpret_cast<float(*)[32]>(&s[0][0]);
+      float (&dpd)[32] = *reinterpret_cast<float(*)[32]>(&dp[0][0]);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_m64n64k16_ss(sd, make_smem_desc_sw128(fa0 + k * 32, 16, 1024), make_smem_desc_sw128(sa0 + k * 32, 16, 1024), k != 0);
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_m64n64k16_ss(dpd, make_smem_desc_sw128(fa1 + k * 32, 16, 1024), make_smem_desc_sw128(sa1 + k * 32, 16, 1024), k != 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_operand32(sd);
+      wgmma_fence_operand32(dpd);
+      uint32_t keep[8];
+      if (DKV) {
+        // ---- as attn_bwd_dkv_kernel: rows = keys (f0 + ...), cols = queries (s0r + ...) ----
+        const int k0 = f0, q0 = s0r;
+        if (p.drop_scale != 0.f) dropout_bits(p, bh, k0 + wq * 16, q0, true, keep);
+        const int ww = wq >> 1;                               // mask word of this warp's 16 key rows
+        float pt[8][4];
+#pragma unroll
+        for (int tt = 0; tt < 8; ++tt) {
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int kr = wq * 16 + gr + (e >> 1) * 8;
+            const int qi = q0 + tt * 8 + 2 * c + (e & 1);
+            const bool qin = qi < p.Lq;
+            const float lse_q = qin ? p.lse[bh * p.Lq + qi] * LOG2E : INFINITY;
+            const float dlt_q = qin ? p.delta[bh * p.Lq + qi] : 0.f;
+            bool vis = (k0 + kr < p.Lk);
+            if (flag == 1) {
+              const int wi = (k0 >> 5) + ww;
+              const uint32_t mw = (qin && wi < p.mask_words) ? __ldg(p.mask + static_cast<long long>(qi) * p.mask_words + wi) : 0u;
+              vis = vis && ((mw >> (kr & 31)) & 1u);
+            }
+            const float pv = vis ? exp2f(s[tt][e] * sc - lse_q) : 0.f;
+            float dpv = dp[tt][e];
+            float pdrop = pv;
+            if (p.drop_scale != 0.f) {
+              const bool kp = (keep[tt] >> e) & 1u;
+              pdrop = kp ? pv * p.drop_scale : 0.f;
+              dpv = kp ? dpv * p.drop_scale : 0.f;
+            }
+            pt[tt][e] = pdrop;
+            s[tt][e] = pv * (dpv - dlt_q);
+          }
+        }
+        uint32_t pa[4][4], da[4][4];
+        c_to_a(pt, pa);
+        c_to_a(s, da);
+        float (&dkd)[32] = *reinterpret_cast<float(*)[32]>(&acc0[0][0]);
+        float (&dvd)[32] = *reinterpret_cast<float(*)[32]>(&acc1[0][0]);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) wgmma_m64n64k16_rs_tb(dvd, pa[kk], make_smem_desc_sw128(sa1 + kk * 2048, 8192, 1024));
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) wgmma_m64n64k16_rs_tb(dkd, da[kk], make_smem_desc_sw128(sa0 + kk * 2048, 8192, 1024));
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_operand32(dkd);
+        wgmma_fence_operand32(dvd);
+      } else {
+        // ---- as attn_bwd_dq_kernel: rows = queries (f0 + ...), cols = keys (s0r + ...) ----
+        const int q0 = f0, k0 = s0r;
+        uint32_t w[2][2] = {{0xffffffffu, 0xffffffffu}, {0xffffffffu, 0xffffffffu}};
+        if (flag == 1) {
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            const int row = q0 + wq * 16 + gr + r * 8;
+#pragma unroll
+            for (int ww = 0; ww < 2; ++ww) {
+              const int wi = t * 2 + ww;
+              w[r][ww] = (row < p.Lq && wi < p.mask_words) ? p.mask[static_cast<long long>(row) * p.mask_words + wi] : 0u;
+            }
+          }
+        }
+        if (p.drop_scale != 0.f) dropout_bits(p, bh, q0 + wq * 16, k0, false, keep);
+#pragma unroll
+        for (int tt = 0; tt < 8; ++tt) {
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int r = e >> 1;
+            const int kk = tt * 8 + 2 * c + (e & 1);
+            bool vis = (k0 + kk < p.Lk);
+            if (flag == 1) vis = vis && ((w[r][kk >> 5] >> (kk & 31)) & 1u);
+            const float pv = vis ? exp2f(s[tt][e] * sc - lse2[r]) : 0.f;
+            float dpv = dp[tt][e];
+            if (p.drop_scale != 0.f) dpv = ((keep[tt] >> e) & 1u) ? dpv * p.drop_scale : 0.f;
+            s[tt][e] = pv * (dpv - dlt[r]);
+          }
+        }
+        uint32_t da[4][4];
+        c_to_a(s, da);
+        float (&dqd)[32] = *reinterpret_cast<float(*)[32]>(&acc0[0][0]);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) wgmma_m64n64k16_rs_tb(dqd, da[kk], make_smem_desc_sw128(sa0 + kk * 2048, 8192, 1024));
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_operand32(dqd);
+      }
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[st]);
+    if (++st == WF_STAGES) { st = 0; ph ^= 1; }
+  }
+  if (g == 1 && !has1) return;
+
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int row = f0 + wq * 16 + gr + r * 8;
+    if (DKV) {
+      if (row < p.Lk) {
+        bf16* dkd = p.dk + b * p.dk_sb + static_cast<long long>(row) * p.dk_ss + h * p.dk_sh;
+        bf16* dvd = p.dv + b * p.dv_sb + static_cast<long long>(row) * p.dv_ss + h * p.dv_sh;
+#pragma unroll
+        for (int tt = 0; tt < 8; ++tt) {
+          *reinterpret_cast<uint32_t*>(dkd + tt * 8 + 2 * c) = pack_bf16x2(acc0[tt][2 * r] * p.scale, acc0[tt][2 * r + 1] * p.scale);
+          *reinterpret_cast<uint32_t*>(dvd + tt * 8 + 2 * c) = pack_bf16x2(acc1[tt][2 * r], acc1[tt][2 * r + 1]);
+        }
+      }
+    } else if (row < p.Lq) {
+      bf16* dst = p.dq + b * p.dq_sb + static_cast<long long>(row) * p.dq_ss + h * p.dq_sh;
+#pragma unroll
+      for (int tt = 0; tt < 8; ++tt)
+        *reinterpret_cast<uint32_t*>(dst + tt * 8 + 2 * c) = pack_bf16x2(acc0[tt][2 * r] * p.scale, acc0[tt][2 * r + 1] * p.scale);
+    }
+  }
+}
+constexpr int WB_SMEM = 1024 + 4 * 8192 + WF_STAGES * 2 * 8192 + 128;
+
 // ===================================================== mask tiles =================================================
 __global__ void attn_mask_tiles_kernel(const uint32_t* __restrict__ mask, int mask_words, int Lq, int Lk, int nkt,
                                        uint8_t* __restrict__ flags) {
@@ -589,16 +1016,54 @@ static bool attn_small_enabled() {
   static const bool on = [] { const char* e = getenv("DVLA_ATTN_SMALL"); return !(e && e[0] == '0'); }();   // thread-safe init
   return on;
 }
-int attn_fwd_ws_dispatch(const dvla_attn_fwd_args* a, cudaStream_t s, long long q_rows);   // attention_fwd_ws.cu (tcgen05, warp-specialised)
 
-// 0 = auto (warp-specialised tcgen05 kernel for Lq >= 96, SIMT row kernel for Lq <= 32 without mask / dropout, mma.sync
-// kernel otherwise), 1 = mma.sync everywhere, 3 = warp-specialised tcgen05 kernel whenever expressible
-static int attn_fwd_mode() {
-  static const int mode = [] {
-    const char* e = getenv("DVLA_ATTN_FWD");
-    return (e && !strcmp(e, "legacy")) ? 1 : (e && !strcmp(e, "ws")) ? 3 : 0;
-  }();
-  return mode;
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+EncodeTiledFn get_encode_fn_shared();   // gemm_sm90.cu
+
+// [B, L, H, 64] strided view -> 4-D tensor map with 64 x 64 boxes, 128-byte swizzle (the layout the wgmma descriptors
+// expect); seq and head dims are ordered so that the strides ascend.
+static bool make_attn_tmap(CUtensorMap* out, const void* base, long long L, long long H, long long B, long long ss,
+                           long long sh, long long sb, int* head_inner) {
+  EncodeTiledFn fn = get_encode_fn_shared();
+  if (!fn) { set_error("cuTensorMapEncodeTiled entry point not found"); return false; }
+  *head_inner = (sh <= ss) ? 1 : 0;
+  cuuint64_t dims[4]; cuuint64_t strides[3]; cuuint32_t box[4]; cuuint32_t estr[4] = {1, 1, 1, 1};
+  dims[0] = 64; box[0] = 64;
+  if (*head_inner) { dims[1] = H; dims[2] = L; strides[0] = sh * 2; strides[1] = ss * 2; box[1] = 1; box[2] = 64; }
+  else             { dims[1] = L; dims[2] = H; strides[0] = ss * 2; strides[1] = sh * 2; box[1] = 64; box[2] = 1; }
+  dims[3] = B; box[3] = 1;
+  strides[2] = (B > 1 ? sb : (long long)dims[1] * dims[2] * 64) * 2;
+  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("attn tensor map encode failed (%d): L=%lld H=%lld B=%lld ss=%lld sh=%lld sb=%lld", (int)r, L, H, B, ss, sh, sb);
+    return false;
+  }
+  return true;
+}
+
+// Strides a tensor map can express: positive, distinct seq / head strides, a head's rows not overlapping the next head.
+static bool tmap_strides_ok(long long L, long long H, long long B, long long ss, long long sh, long long sb) {
+  if (ss <= 0 || sh <= 0 || ss == sh || (B > 1 && sb <= 0)) return false;
+  return (sh < ss) ? (sh >= 64 && ss >= sh * H) : (ss >= 64 && sh >= ss * L);
+}
+
+static int attn_fwd_wgmma_launch(const dvla_attn_fwd_args* a, const AttnParams& p, cudaStream_t s) {
+  WgmmaFwdMaps tm;
+  if (!make_attn_tmap(&tm.q, a->q, a->Lq, a->H, a->B, a->q_ss, a->q_sh, a->q_sb, &tm.q_head_inner) ||
+      !make_attn_tmap(&tm.k, a->k, a->Lk, a->H, a->B, a->k_ss, a->k_sh, a->k_sb, &tm.k_head_inner) ||
+      !make_attn_tmap(&tm.v, a->v, a->Lk, a->H, a->B, a->v_ss, a->v_sh, a->v_sb, &tm.v_head_inner))
+    return DVLA_ERR_CUDA;
+  static std::once_flag once;
+  static cudaError_t attr_err = cudaSuccess;
+  std::call_once(once, [] { attr_err = cudaFuncSetAttribute(attn_fwd_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WF_SMEM); });
+  if (attr_err != cudaSuccess) { set_error("attn_fwd_wgmma smem attribute: %s", cudaGetErrorString(attr_err)); return DVLA_ERR_CUDA; }
+  attn_fwd_wgmma_kernel<<<dim3(p.H, p.B, (p.nqt + 1) / 2), WF_THREADS, WF_SMEM, s>>>(tm, p);
+  DVLA_CHECK_LAUNCH("attn_fwd_wgmma");
+  return DVLA_OK;
 }
 
 int attn_fwd_dispatch(const dvla_attn_fwd_args* a, cudaStream_t s) {
@@ -612,7 +1077,6 @@ int attn_fwd_dispatch(const dvla_attn_fwd_args* a, cudaStream_t s) {
   if (a->H > 65535 || a->B > 65535) { set_error("attn_fwd: B,H must be <= 65535"); return DVLA_ERR_UNSUPPORTED; }
   if (a->mask && a->mask_words * 32 < a->Lk) { set_error("attn_fwd: mask_words too small"); return DVLA_ERR_INVALID; }
   if (a->mask && !a->tile_flags) { set_error("attn_fwd: mask given without tile_flags"); return DVLA_ERR_INVALID; }
-  const int mode = attn_fwd_mode();
   if (a->key_bias) {
     if (!attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p)) {
       set_error("attn_fwd: key_bias needs the short-sequence kernels (Lq <= 32, Lk <= 64, no mask, no dropout)");
@@ -620,7 +1084,7 @@ int attn_fwd_dispatch(const dvla_attn_fwd_args* a, cudaStream_t s) {
     }
     return attn_small_fwd_dispatch(a, s);
   }
-  if (mode == 0 && attn_small_enabled() && attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p))
+  if (attn_small_enabled() && attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p))
     return attn_small_fwd_dispatch(a, s);
   AttnParams p;
   memset(&p, 0, sizeof(p));
@@ -637,28 +1101,26 @@ int attn_fwd_dispatch(const dvla_attn_fwd_args* a, cudaStream_t s) {
     p.drop_seed = a->dropout_seed;
     p.drop_seed_ptr = a->dropout_seed_ptr;
   }
-  if (mode == 3 || (mode == 0 && a->Lq >= 96)) {
-    // warp-specialised tcgen05 kernel on 256-query CTAs.  (Sending a short remainder of <= 64 rows to the mma.sync kernel
-    // instead of a latency-bound CTA was measured and lost: profiles/r1_notes.md.)
-    const int rc = attn_fwd_ws_dispatch(a, s, a->Lq);
-    if (rc != DVLA_ERR_UNSUPPORTED) return rc;
-  }
+  // wgmma + TMA for the long sequences (backbone, ViT, decoders); the mma.sync kernel for short query blocks and strides a
+  // tensor map cannot express
+  if (a->Lq >= 96 && tmap_strides_ok(a->Lq, a->H, a->B, a->q_ss, a->q_sh, a->q_sb) &&
+      tmap_strides_ok(a->Lk, a->H, a->B, a->k_ss, a->k_sh, a->k_sb) && tmap_strides_ok(a->Lk, a->H, a->B, a->v_ss, a->v_sh, a->v_sb))
+    return attn_fwd_wgmma_launch(a, p, s);
   attn_fwd_kernel<<<dim3(p.nqt, p.H, p.B), 128, 0, s>>>(p);
   DVLA_CHECK_LAUNCH("attn_fwd");
   return DVLA_OK;
 }
 
-int attn_bwd_ws_dispatch(const dvla_attn_bwd_args* a, const uint32_t* mask_t, int mask_t_words, cudaStream_t s, long long q_rows,
-                         long long k_rows);    // attention_bwd_ws.cu
-
-// 0 = auto (warp-specialised tcgen05 kernels when both sequences are >= 96 long, SIMT row kernels for Lq <= 32 without
-// mask / dropout, mma.sync kernels otherwise), 1 = mma.sync kernels everywhere, 4 = warp-specialised whenever expressible
-static int attn_bwd_mode() {
-  static const int mode = [] {
-    const char* e = getenv("DVLA_ATTN_BWD");
-    return (e && !strcmp(e, "legacy")) ? 1 : (e && !strcmp(e, "ws")) ? 4 : 0;
-  }();
-  return mode;
+template <bool DKV>
+static int attn_bwd_wgmma_launch(const WgmmaBwdMaps& tm, const AttnParams& p, cudaStream_t s) {
+  static std::once_flag once;
+  static cudaError_t attr_err = cudaSuccess;
+  std::call_once(once, [] { attr_err = cudaFuncSetAttribute(attn_bwd_wgmma_kernel<DKV>, cudaFuncAttributeMaxDynamicSharedMemorySize, WB_SMEM); });
+  if (attr_err != cudaSuccess) { set_error("attn_bwd_wgmma smem attribute: %s", cudaGetErrorString(attr_err)); return DVLA_ERR_CUDA; }
+  const int nf = DKV ? p.nkt : p.nqt;
+  attn_bwd_wgmma_kernel<DKV><<<dim3(p.H, p.B, (nf + 1) / 2), WF_THREADS, WB_SMEM, s>>>(tm, p);
+  DVLA_CHECK_LAUNCH(DKV ? "attn_bwd_dkv_wgmma" : "attn_bwd_dq_wgmma");
+  return DVLA_OK;
 }
 
 int attn_bwd_dispatch(const dvla_attn_bwd_args* a, cudaStream_t s) {
@@ -693,7 +1155,6 @@ int attn_bwd_dispatch(const dvla_attn_bwd_args* a, cudaStream_t s) {
     p.drop_seed = a->dropout_seed;
     p.drop_seed_ptr = a->dropout_seed_ptr;
   }
-  const int bmode = attn_bwd_mode();
   if (a->key_bias) {
     if (!attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p)) {
       set_error("attn_bwd: key_bias needs the short-sequence kernels (Lq <= 32, Lk <= 64, no mask, no dropout)");
@@ -701,15 +1162,27 @@ int attn_bwd_dispatch(const dvla_attn_bwd_args* a, cudaStream_t s) {
     }
     return attn_small_bwd_dispatch(a, s);
   }
-  if (bmode == 0 && attn_small_enabled() && attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p))
+  if (attn_small_enabled() && attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p))
     return attn_small_bwd_dispatch(a, s);          // writes delta itself
   const long long rows = (long long)p.B * p.H * p.Lq;
   attn_delta_kernel<<<(unsigned)((rows * 8 + 255) / 256), 256, 0, s>>>(p);
   DVLA_CHECK_LAUNCH("attn_delta");
-  if (bmode == 4 || (bmode == 0 && a->Lq >= 96 && a->Lk >= 96)) {
-    // warp-specialised tcgen05 kernels, 2 CTAs / SM (attention_bwd_ws.cu)
-    const int rc = attn_bwd_ws_dispatch(a, a->mask_t, a->mask_t_words, s, a->Lq, a->Lk);
-    if (rc != DVLA_ERR_UNSUPPORTED) return rc;
+  // wgmma + TMA when both sequences are long and every operand is tensor-map addressable; mma.sync kernels otherwise
+  if (a->Lq >= 96 && a->Lk >= 96 && a->B <= 65535 && a->H <= 65535 &&
+      tmap_strides_ok(a->Lq, a->H, a->B, a->q_ss, a->q_sh, a->q_sb) && tmap_strides_ok(a->Lq, a->H, a->B, a->do_ss, a->do_sh, a->do_sb) &&
+      tmap_strides_ok(a->Lk, a->H, a->B, a->k_ss, a->k_sh, a->k_sb) && tmap_strides_ok(a->Lk, a->H, a->B, a->v_ss, a->v_sh, a->v_sb)) {
+    CUtensorMap tq, tdo, tk, tv;
+    int hq, hdo, hk, hv;
+    if (!make_attn_tmap(&tq, a->q, a->Lq, a->H, a->B, a->q_ss, a->q_sh, a->q_sb, &hq) ||
+        !make_attn_tmap(&tdo, a->d_o, a->Lq, a->H, a->B, a->do_ss, a->do_sh, a->do_sb, &hdo) ||
+        !make_attn_tmap(&tk, a->k, a->Lk, a->H, a->B, a->k_ss, a->k_sh, a->k_sb, &hk) ||
+        !make_attn_tmap(&tv, a->v, a->Lk, a->H, a->B, a->v_ss, a->v_sh, a->v_sb, &hv))
+      return DVLA_ERR_CUDA;
+    const WgmmaBwdMaps dkv{tk, tv, tq, tdo, hk, hv, hq, hdo};
+    const WgmmaBwdMaps dq{tq, tdo, tk, tv, hq, hdo, hk, hv};
+    const int rc = attn_bwd_wgmma_launch<true>(dkv, p, s);
+    if (rc != DVLA_OK) return rc;
+    return attn_bwd_wgmma_launch<false>(dq, p, s);
   }
   attn_bwd_dkv_kernel<<<dim3(p.nkt, p.H, p.B), 128, 0, s>>>(p);
   DVLA_CHECK_LAUNCH("attn_bwd_dkv");

@@ -180,9 +180,8 @@ __global__ void __launch_bounds__(256) attn_small_bwd_dkv_kernel(const SmallPara
 
 }  // namespace
 
-// Measured on B200 (profiles/r2_kernel_check_attn.log): 20 us fwd / 36 us bwd for the DiT shape (7680 (b,h) x 6x6), but the
-// serial key loop loses to the mma.sync kernel once there are hundreds of keys per row (16x212: 138 us fwd; 10x265: 630 us),
-// so the row kernels take the short-key case only.
+// The serial key loop of these row kernels loses to the mma.sync kernel once there are hundreds of keys per row, so they
+// take the short-key case only (the DiT blocks: 6 x 6 per (b,h)).
 constexpr int SMALL_MAX_LQ = 32;
 constexpr int SMALL_MAX_LK = 64;
 

@@ -1,4 +1,4 @@
-// extern "C" entry points of libdvla_sm100.so (declared in include/dvla.h): argument validation, error text,
+// extern "C" entry points of libdvla_sm90.so (declared in include/dvla.h): argument validation, error text,
 // launch accounting.  No torch types cross this boundary.
 #include <atomic>
 #include <stdarg.h>
@@ -27,7 +27,7 @@ int num_sms() {
   static const int n = [] {
     int dev = 0, v = 0;
     cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;   // H100 SXM
     return v;
   }();
   const int b = g_sm_budget.load(std::memory_order_relaxed);

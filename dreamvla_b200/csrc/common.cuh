@@ -1,6 +1,6 @@
-// Shared device helpers for the sm_100a kernels: mbarrier, TMA, tcgen05/TMEM PTX wrappers,
+// Shared device helpers for the sm_90a kernels: mbarrier, TMA, wgmma PTX wrappers,
 // bf16 packing, warp reductions and a counter-based RNG for dropout.
-// Everything here is hand-written inline PTX for sm_100a (no CUTLASS dependency in the build).
+// Everything here is hand-written inline PTX for sm_90a (no CUTLASS dependency in the build).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -50,6 +50,9 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
+// kReport = false: the same watchdog without the diagnostic printf.  printf is a function call, and a call anywhere in a
+// function that issues wgmma makes ptxas serialise every wgmma of that function.
+template <bool kReport = true>
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   uint32_t spins = 0;
@@ -59,12 +62,18 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       const long long now = clock64();
       if (t0 == 0) t0 = now;
       else if (now - t0 > DVLA_WATCHDOG_CYCLES) {
-        printf("dvla: mbarrier watchdog (block %d thread %d parity %u)\n", blockIdx.x, threadIdx.x, parity);
+        if (kReport) printf("dvla: mbarrier watchdog (block %d thread %d parity %u)\n", blockIdx.x, threadIdx.x, parity);
         __trap();
       }
     }
   }
 }
+
+// Hand registers between warpgroups of a warp-specialised kernel (per-warpgroup register budget, sm_90a).
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // ---------------------------------------------------------------------------------------------
 // TMA (cp.async.bulk.tensor), 2-D and 3-D tiled loads into shared memory, completion on mbarrier
@@ -88,122 +97,89 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
 }
 
 // ---------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// wgmma (sm_90a warpgroup MMA): D[64 x 128] fp32 in registers (+)= A[smem desc] * B[smem desc], bf16 inputs.
+// Issued by all 128 threads of a warpgroup.
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {  // whole warp, .sync.aligned
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Keeps the compiler from moving reads or writes of the accumulator across a wgmma_wait.
+__device__ __forceinline__ void wgmma_fence_operand(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc]; bf16 inputs, fp32 accumulate; issued by ONE thread.
-__device__ __forceinline__ void umma_bf16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
+// Accumulator layout (per warp w of the warpgroup, lane l): d[4*j + 2*h + e] is row 16*w + l/4 + 8*h, column
+// 8*j + 2*(l%4) + e.  TA / TB = 1 reads that operand MN-major (transposed) from shared memory.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128k16_bf16(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(TA), "n"(TB)
       : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
 }
 
-// ---- cta_group::2 (CTA pair) variants --------------------------------------------------------------------------------
-// In a 2-CTA cluster the shared::cluster address of an object in CTA r is (cta-local address | r << 24); masking bit 24
-// addresses the leader (rank 0) copy.
-constexpr uint32_t PEER_BIT_MASK = 0xFEFFFFFFu;
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// TMA load executed by either CTA of the pair into ITS OWN smem, completing tx bytes on the LEADER's mbarrier.
-__device__ __forceinline__ void tma_load_2d_2cta(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & PEER_BIT_MASK), "r"(c0), "r"(c1)
-      : "memory");
-}
-// arrive on the LEADER CTA's copy of `bar` (callable from either CTA)
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & PEER_BIT_MASK) : "memory");
-}
-__device__ __forceinline__ void umma_bf16_ss_2cta(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                  uint32_t accumulate) {
+// D[64 x 64] fp32 (+)= A[smem desc] * B[smem desc]; both operands K-major.
+__device__ __forceinline__ void wgmma_m64n64k16_ss(float (&d)[32], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate)
       : "memory");
 }
-// arrive (once all prior MMAs of this thread completed) on `bar` in BOTH CTAs of the pair
-__device__ __forceinline__ void umma_commit_2cta(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"(static_cast<uint16_t>(3))
-               : "memory");
-}
-
-// TMEM -> registers: 32 lanes x 32 consecutive fp32 columns; thread t of the warp receives lane (base_lane + t).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
+// D[64 x 64] fp32 += A[registers] * B[smem desc, MN-major]; A is the bf16 fragment of mma.sync m16n8k16 for this warp's 16
+// rows (a[0..3]), so an accumulator of this shape converts to the next A operand without leaving registers.
+__device__ __forceinline__ void wgmma_m64n64k16_rs_tb(float (&d)[32], const uint32_t (&a)[4], uint64_t desc_b) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, 1, 1, 1, 1;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b)
       : "memory");
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_fence_operand32(float (&d)[32]) {
+#pragma unroll
+  for (int i = 0; i < 32; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
 
-// UMMA shared-memory matrix descriptor (sm_100 "version 1"), 128-byte swizzle.
-//   bits [0,14)  start address >> 4      bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4 bits [46,48) version = 1     bits [61,64) layout type (2 = SWIZZLE_128B)
-// K-major tile  (rows x 64 bf16, one 128 B swizzle row per matrix row): SBO = 1024 (8 rows), LBO unused (=1).
+// wgmma shared-memory matrix descriptor (sm_90), 128-byte swizzle.
+//   bits [0,14) start address >> 4    bits [16,30) leading byte offset >> 4    bits [32,46) stride byte offset >> 4
+//   bits [62,64) layout type (1 = SWIZZLE_128B).  Tiles are 1024-byte aligned, so the base-offset field stays 0.
+// K-major tile  (rows x 64 bf16, one 128 B swizzle row per matrix row): SBO = 1024 (8 rows), LBO unused.
 // MN-major tile (64-wide MN atoms, K rows of 128 B): SBO = 1024 (8 K-rows), LBO = bytes between 64-wide MN atoms.
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
 
-// tcgen05 instruction descriptor for kind::f16: bf16 x bf16 -> fp32.
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, bool a_mn_major, bool b_mn_major) {
-  return (1u << 4)                               // c_format = F32
-         | (1u << 7)                             // a_format = BF16
-         | (1u << 10)                            // b_format = BF16
-         | ((a_mn_major ? 1u : 0u) << 15)        // a_major
-         | ((b_mn_major ? 1u : 0u) << 16)        // b_major
-         | (static_cast<uint32_t>(N >> 3) << 17) // n_dim
-         | (static_cast<uint32_t>(M >> 4) << 24);// m_dim
+// Named barrier over `count` threads (ids 1.. ; 0 is __syncthreads).
+__device__ __forceinline__ void named_barrier_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -232,8 +208,7 @@ __device__ __forceinline__ float warp_max(float v) {
 enum Act : int { ACT_NONE = 0, ACT_GELU_ERF = 1, ACT_GELU_TANH = 2, ACT_QUICK_GELU = 3, ACT_RELU = 4, ACT_SILU = 5 };
 
 // Branch-free approximate reciprocal / exp2 (single MUFU each).  The IEEE variants (`/`, __frcp_rn, expf) compile to a MUFU
-// plus a guarded slow path -- one branch per element -- which made the GEMM epilogue instruction-bound (47 warp
-// instructions per output element in the first ncu capture, profiles/r1_gemm_epilogue_v1.txt).
+// plus a guarded slow path -- one branch per element -- which makes an epilogue of a few flops per element instruction-bound.
 __device__ __forceinline__ float rcp_approx(float x) {
   float r;
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
@@ -362,8 +337,8 @@ __device__ __forceinline__ void act_bwd_mul_n(float (&v)[N], const float (&x)[N]
 
 // Counter-based RNG (Philox-4x32, Salmon et al. SC'11).  One call yields 4 uniform 32-bit words for (seed, offset).
 // 7 rounds: the smallest round count the authors report as passing BigCrush (curand's default of 10 adds margin only);
-// the dropout masks need independent Bernoulli draws, not cryptographic strength, and the RNG is the larger half of the
-// instructions of the attention kernels' dropout path (profiles/r1_notes.md).
+// the dropout masks need independent Bernoulli draws, not cryptographic strength, and the RNG dominates the instructions of
+// the attention kernels' dropout path.
 constexpr int DVLA_PHILOX_ROUNDS = 7;
 __device__ __forceinline__ uint4 philox4x32(uint64_t seed, uint64_t offset) {
   uint32_t k0 = static_cast<uint32_t>(seed), k1 = static_cast<uint32_t>(seed >> 32);

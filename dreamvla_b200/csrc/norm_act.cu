@@ -207,8 +207,8 @@ __global__ void __launch_bounds__(256, 2) layernorm_bwd_kernel(const bf16* __res
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// LayerNorm backward, version 2 (D a multiple of 256, with dgamma/dbeta): the kernel above moves 2.4 TB/s on the decoders'
-// [42400, 1024] tensors (profiles/r2_ncu_hbm.txt: 346 MB in 144 us, 37 % of the HBM peak) because a row costs two dependent
+// LayerNorm backward, version 2 (D a multiple of 256, with dgamma/dbeta): the kernel above is latency-bound on the decoders'
+// [42400, 1024] tensors because a row costs two dependent
 // round trips (x, dy -> reduce -> dres) and its 64 per-lane dgamma/dbeta partials cap residency at 16 warps per SM.  Here the
 // partials live in SHARED memory (one private [2][D] fp32 slab per warp, plain read-modify-write with 16-byte accesses), the
 // residual-branch gradient is fetched with x and dy (one round trip per row); 2 CTAs per SM without spills (3 would need <= 85 registers).

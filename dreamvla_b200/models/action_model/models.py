@@ -1,4 +1,4 @@
-"""DiT action head on sm_100a kernels -- mirror of reference models/action_model/models.py:28-268.
+"""DiT action head on sm_90a kernels -- mirror of reference models/action_model/models.py:28-268.
 
 Plain pre-LN ViT blocks (no adaLN): LayerNorm without affine (eps 1e-6), timm Attention (qkv_bias), Mlp with
 GELU(tanh).  Parameter names follow the reference (x_embedder.linear, t_embedder.mlp.{0,2}, z_embedder.{linear,

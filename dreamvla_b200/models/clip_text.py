@@ -1,4 +1,4 @@
-"""CLIP text tower (openai/CLIP model.py `encode_text`, ViT-B/32 text hyper-parameters) on sm_100a kernels.
+"""CLIP text tower (openai/CLIP model.py `encode_text`, ViT-B/32 text hyper-parameters) on sm_90a kernels.
 
 Boundary input of the hot path (dreamvla_model.py:643-649; SURVEY §2.3 k17): frozen, no_grad.  openai/CLIP is not
 installable offline, so `load()` returns a random-initialised tower with CLIP's parameter names

@@ -1,12 +1,12 @@
-"""DreamVLA on sm_100a kernels -- drop-in mirror of reference models/dreamvla_model.py:122-991.
+"""DreamVLA on sm_90a kernels -- drop-in mirror of reference models/dreamvla_model.py:122-991.
 
 Same constructor kwargs, `forward(image_primary, image_wrist, state, text_token, action=None, track_infos=None,
 action_label=None, mode='train')` -> the same 10-tuple, same parameter names / shapes (state_dict-compatible, incl. HF
 Conv1D [in,out] weights), same attributes read by the entry points (`image_processor`, `clip_model`, `vision_encoder`,
 `perceiver_resampler`, `transformer_backbone`, `*_decoder`, `action_model`, `_init_model_type()`, `sequence_length`).
 
-What differs, by design (B200-first, results identical up to bf16 rounding):
-  * every Linear/LayerNorm/attention runs on libdvla_sm100.so (tcgen05 GEMM with fused bias/act/residual/dropout
+What differs, by design (H100-first, results identical up to bf16 rounding):
+  * every Linear/LayerNorm/attention runs on libdvla_sm90.so (wgmma GEMM with fused bias/act/residual/dropout
     epilogues, flash attention with the reference's {0,-inf} mask as a bit matrix + tile skipping);
   * both cameras go through the ViT / resampler in ONE batched call (the reference makes two, :672-673,:716-717);
   * the ViT patch-token permutation of random_masking(…, 0.0) is skipped (outputs invariant, see vit_mae.py here);

@@ -1,4 +1,4 @@
-"""Trimmed GPT-2 backbone on sm_100a kernels -- mirror of reference models/gpt2.py:22-480.
+"""Trimmed GPT-2 backbone on sm_90a kernels -- mirror of reference models/gpt2.py:22-480.
 
 Takes `inputs_embeds` [B, L, D] and the additive {0,-inf} attention mask of dreamvla_model.py:25-66; both
 `attn_implementation` values of the reference ("eager" gpt2.py:61-84, "sdpa" gpt2.py:196-284) map to the same

@@ -1,6 +1,6 @@
-"""Building blocks with the parameter names / shapes of the reference's third-party layers, forward on sm_100a kernels.
+"""Building blocks with the parameter names / shapes of the reference's third-party layers, forward on sm_90a kernels.
 
-  Linear      == torch.nn.Linear            (weight [out,in])              -> ops.linear (tcgen05 GEMM + fused epilogue)
+  Linear      == torch.nn.Linear            (weight [out,in])              -> ops.linear (wgmma GEMM + fused epilogue)
   Conv1D      == transformers Conv1D        (weight [in,out], gpt2.py:53)  -> ops.linear(weight_kn=True)
   LayerNorm   == torch.nn.LayerNorm                                        -> ops.layer_norm
   Attention / Mlp / Block == timm 0.9.16 vision_transformer.{Attention, Mlp, Block} (names norm1, attn.qkv, attn.proj,
@@ -20,7 +20,7 @@ def _require_bf16(p: torch.Tensor, what: str):
     if p.dtype != torch.bfloat16 or not p.is_cuda:
         raise RuntimeError(
             f"{what}: dreamvla_b200 kernels are bf16/CUDA only (got {p.dtype} on {p.device}); cast the model with "
-            ".bfloat16() and move it to a B200 -- there is no CPU or fp32 fallback path")
+            ".bfloat16() and move it to an H100 -- there is no CPU or fp32 fallback path")
 
 
 class Linear(nn.Linear):

@@ -1,4 +1,4 @@
-"""Flamingo Perceiver resampler on sm_100a kernels -- mirror of reference models/perceiver_resampler.py:11-128.
+"""Flamingo Perceiver resampler on sm_90a kernels -- mirror of reference models/perceiver_resampler.py:11-128.
 
 Parameter names follow the reference (layers.N.0.{norm_media,norm_latents,to_q,to_kv,to_out}, layers.N.1.{0,1,3}, norm).
 Cross-attention over [media ; latents] keys runs in the flash kernel (no materialised `sim`, perceiver_resampler.py:55-57);

@@ -1,4 +1,4 @@
-"""MAE ViT-B/16 encoder on sm_100a kernels -- mirror of reference models/vit_mae.py:55-206 (encoder half only).
+"""MAE ViT-B/16 encoder on sm_90a kernels -- mirror of reference models/vit_mae.py:55-206 (encoder half only).
 
 Only `forward_encoder(x, mask_ratio=0.0)` is on the hot path (dreamvla_model.py:672-673).  The MAE decoder half of the
 reference class (26 M parameters, never executed by DreamVLA) is not instantiated; MAE checkpoints load with

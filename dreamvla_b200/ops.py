@@ -1,4 +1,4 @@
-"""torch.autograd.Function ops backed by libdvla_sm100.so -- the host-side mirror of the reference's PyTorch call sites.
+"""torch.autograd.Function ops backed by libdvla_sm90.so -- the host-side mirror of the reference's PyTorch call sites.
 
 Every op here runs ONLY on the hand-written CUDA kernels (via dreamvla_b200._lib); there is no eager fallback.
 
@@ -164,13 +164,13 @@ class _Linear(torch.autograd.Function):
 
 
 def linear(x, weight, bias=None, *, act=None, residual=None, weight_kn=False, dropout_p=0.0, alpha=1.0):
-    """Fused linear layer on the tcgen05 GEMM.  x [..., K] bf16."""
+    """Fused linear layer on the wgmma GEMM.  x [..., K] bf16."""
     return _apply(_Linear, x, weight, bias, residual, ACT_IDS[act] if not isinstance(act, int) else act, weight_kn,
                          float(dropout_p), float(alpha))
 
 
 # A/B switch: apply act'(pre) in the epilogue of the second layer's dgrad GEMM (DVLA_FUSE_ACT_BWD=1) instead of the separate
-# HBM-bound act_bwd kernel; see profiles/r1_notes.md for the measurements behind the default.
+# HBM-bound act_bwd kernel.
 _FUSE_ACT_BWD = os.environ.get("DVLA_FUSE_ACT_BWD", "0") == "1"
 
 
@@ -204,9 +204,8 @@ class _MLP(torch.autograd.Function):
         dy2 = _as2d(_bf16c(dy))
         d_res = dy.view(res_shape) if res_shape is not None and ctx.needs_input_grad[5] else None
         dz2 = L.dropout(dy2, dropout_p, seed, seed_ptr=seed_counter(dy2.device)) if dropout_p > 0 else dy2
-        # (dZ2 W2) * act'(pre).  The GEMM can apply act' in its epilogue (aux_in): measured +18 % GEMM time with 8 epilogue
-        # warps per CTA and still no gain with 16 (104.9 vs 104.3 ms/step, profiles/r1_notes.md), so the HBM-bound
-        # elementwise kernel stays the default.
+        # (dZ2 W2) * act'(pre).  The GEMM can apply act' in its epilogue (aux_in); the act' evaluation then sits on the
+        # GEMM's critical path, so the HBM-bound elementwise kernel is the default.
         b1_done = False
         if _FUSE_ACT_BWD:
             dh = L.gemm(dz2, w2, b_mn=not weight_kn, aux_in=aux, act=act)
@@ -334,7 +333,6 @@ class AttnMask:
     def __init__(self, visible_bool: torch.Tensor, device):
         self.Lq, self.Lk = visible_bool.shape
         self.bits = self.pack_bits(visible_bool).to(device).contiguous()
-        self.bits_t = self.pack_bits(visible_bool.t().contiguous()).to(device).contiguous()   # [Lk, ceil(Lq/32)]
         self.flags = L.attn_mask_tiles(self.bits, self.Lq, self.Lk)
 
     @staticmethod
@@ -408,7 +406,7 @@ class _Attention(torch.autograd.Function):
         L.attn_bwd(q, k, v, o, d_o, lse, scale, dq, dk, dv, mask.bits if mask is not None else None,
                    mask.flags if mask is not None else None, dropout_p, seed,
                    dropout_seed_ptr=seed_counter(q.device) if dropout_p > 0 else None,
-                   mask_bits_t=mask.bits_t if mask is not None else None, key_bias=key_bias)
+                   key_bias=key_bias)
         return dq, dk, dv, None, None, None, None
 
 
@@ -442,8 +440,7 @@ class _FusedQKVAttention(torch.autograd.Function):
         dqkv = torch.empty_like(qkv)
         L.attn_bwd(qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2], o, d_o, lse, scale, dqkv[:, :, 0], dqkv[:, :, 1],
                    dqkv[:, :, 2], mask.bits if mask is not None else None, mask.flags if mask is not None else None,
-                   dropout_p, seed, dropout_seed_ptr=seed_counter(qkv.device) if dropout_p > 0 else None,
-                   mask_bits_t=mask.bits_t if mask is not None else None)
+                   dropout_p, seed, dropout_seed_ptr=seed_counter(qkv.device) if dropout_p > 0 else None)
         return dqkv, None, None, None
 
 

@@ -64,7 +64,7 @@ _EXTRA = [("--synthetic_steps", int, 0), ("--cuda_graph", "flag", False), ("--sy
 
 
 def get_parser() -> argparse.ArgumentParser:
-    parser = argparse.ArgumentParser(description="DreamVLA hot path on B200 (reference-compatible flags)")
+    parser = argparse.ArgumentParser(description="DreamVLA hot path on H100 (reference-compatible flags)")
     for spec in _FLAGS + _EXTRA:
         name, typ, default = spec[0], spec[1], spec[2]
         if typ == "flag":

@@ -45,7 +45,7 @@ def init_distributed_device(args):
     if not hasattr(args, "world_size"):
         args.local_rank, args.rank, args.world_size = world_info_from_env()
     if not torch.cuda.is_available():
-        raise RuntimeError("dreamvla_b200 needs a CUDA device (B200); there is no CPU path")
+        raise RuntimeError("dreamvla_b200 needs a CUDA device (H100); there is no CPU path")
     device = torch.device("cuda", args.local_rank)
     torch.cuda.set_device(device)
     if args.world_size > 1:

@@ -1,4 +1,4 @@
-"""Train step of the hot path -- B200-native mirror of reference utils/train_utils.py:59-726 (`train_one_epoch_calvin`).
+"""Train step of the hot path -- H100-native mirror of reference utils/train_utils.py:59-726 (`train_one_epoch_calvin`).
 
 Reference step (train_utils.py:94-608): unpack the 13-tuple batch, build labels, forward, seven losses with weights
 (1.0 arm, 0.01 gripper, 0.1 image, 0.001 depth, 0.1 traj(x0.1), 0.01 dino, 0.01 sam, :585), `/accum`, backward (DDP
@@ -419,8 +419,8 @@ class TrainStep:
         self.last_terms = {}
         # The gradient segments that complete early (heads/decoders/DiT, then the second half of the backbone) are all-reduced
         # from backward hooks on the communication stream, overlapping the rest of the backward pass; the remainder follows
-        # after backward.  Validated on 2 GPUs against one flat all-reduce (tools/ddp_overlap_check.py,
-        # profiles/r1_ddp_overlap_check.log), eagerly and inside the captured step.  DVLA_AR_OVERLAP=0 turns it off.
+        # after backward.  tools/ddp_overlap_check.py compares it on 2 GPUs against one flat all-reduce, eagerly and inside the
+        # captured step.  DVLA_AR_OVERLAP=0 turns it off.
         self.overlap = world_size > 1 and os.environ.get("DVLA_AR_OVERLAP", "1") != "0"
         self._reduced_upto = 0
         # while gradient segments are in flight the persistent GEMMs of backward are sized for the SMs NCCL leaves free
@@ -711,7 +711,7 @@ def prefetch_to_device(loader, device, to_host_dict=None, dtype=torch.bfloat16, 
             # HOST-side wait for the step that read this slot's buffers (it finished long ago unless the host runs more than a
             # step ahead).  A device-side wait (copy_stream.wait_event) would park the copy in the stream's hardware queue
             # until the event fires; with the overlapped NCCL all-reduces of the data-parallel step in flight, copies parked
-            # or released at arbitrary points of the step cost 8-26 ms per step at 4-8 GPUs (profiles/r2_multi_gpu.md)
+            # or released at arbitrary points of the step delay the step by an unpredictable amount
             slot.consumed.synchronize()
         with torch.cuda.stream(copy_stream):
             dev = slot.fill(to_host_dict(item), device, dtype)

@@ -1,4 +1,4 @@
-/* libdvla_sm100.so -- C ABI of the B200-native DreamVLA hot path.
+/* libdvla_sm90.so -- C ABI of the H100-native (sm_90a) DreamVLA hot path.
  *
  * The reference (Zhangwenyao1/DreamVLA @ 7145258) is 100 % Python and has no FFI of its own; every entry point
  * below replaces a PyTorch call site of the reference, cited as <file>:<line> into the reference tree.
@@ -44,7 +44,7 @@ int64_t dvla_launch_count(void);
  * Replaces: torch.nn.Linear / timm Mlp / timm Attention.qkv,proj (models/vit_mae.py:73-75, dreamvla_model.py:348-433,
  * action_model/models.py:130-134), HF Conv1D addmm (models/gpt2.py:53-54,292-293), the perceiver projections
  * (models/perceiver_resampler.py:14-17,31-33) and their autograd dgrad/wgrad.
- * Hot path: persistent warp-specialised tcgen05.mma (TMEM accumulators, TMA-fed 128B-swizzled smem ring).
+ * Hot path: persistent warp-specialised wgmma (register accumulators, TMA-fed 128B-swizzled smem ring).
  * Operands whose strides/pointers are not 16-byte aligned run on a SIMT kernel of the same semantics.
  * ------------------------------------------------------------------------------------------------------------- */
 typedef struct {
@@ -79,8 +79,8 @@ int dvla_gemm(const dvla_gemm_args* args, void* stream);
  * Work unit u of the persistent kernels covers k-blocks [kb0, kb1) of 64 of output tile `tile` (m fastest); tail_slot >= 0
  * marks a K-split tail unit (partial sums through the workspace), split its index among the tile's splits. */
 typedef struct dvla_gemm_plan_info {
-  int32_t kernel;                 /* 0 SIMT thread-per-8-outputs, 1 SIMT warp-per-8-outputs, 2 tcgen05 one CTA, 3 tcgen05 CTA pair */
-  int32_t tile_m, tile_n;         /* output tile of one CTA (pair): 128 x {128, 256} or 256 x 256 */
+  int32_t kernel;                 /* 0 SIMT thread-per-8-outputs, 1 SIMT warp-per-8-outputs, 2 wgmma (3 is not used on sm_90) */
+  int32_t tile_m, tile_n;         /* output tile of one CTA: 128 x 128 */
   int32_t m_tiles, n_tiles, k_blocks;
   int32_t k_splits, kb_per_split, atomic_out;     /* uniform split-K (weight gradients), bf16 red.global.add when atomic_out */
   int32_t tail_first, tail_splits, tail_kbps;     /* K-split tail: tiles >= tail_first are cut into tail_splits k-ranges */
@@ -171,7 +171,7 @@ typedef struct {
   float dropout_p; uint64_t dropout_seed;
   const uint64_t* dropout_seed_ptr;
   const uint32_t* mask_t;     /* optional TRANSPOSED bit matrix [Lk, mask_t_words] (bit i%32 of word i/32 of row j = pair (i,j)
-                                 visible); lets the tcgen05 dK/dV kernel read a key row's query bits contiguously */
+                                 visible); accepted for ABI compatibility, not read by the sm_90 kernels */
   int32_t mask_t_words;
   const float* key_bias;      /* as in dvla_attn_fwd_args (a constant: receives no gradient) */
 } dvla_attn_bwd_args;

@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE (never imported by dreamvla_b200/): CPU restatement of the two device-side collator pieces of SURVEY.md
 8f-2 -- the reference's `RandomShiftsAug` (utils/data_utils.py:326-383) and the NEAREST depth resize of `depth_image_fn`
-(utils/data_utils.py:3588-3603) -- pinned against the reference's own code by tests/test_augment_cpu.py (the class / function
-bodies are executed straight from /root/reference when it is present, and through tests/golden/augment.pt otherwise).
+(utils/data_utils.py:3588-3603) -- pinned against the reference's own code by tests/test_augment_cpu.py (through the reference
+outputs recorded in tests/golden/augment.pt and tests/golden/reference_checks.pt).
 
 Two forms of the augmentation are given:
   * `random_shifts_grid_sample` follows the reference line by line: replicate pad, fp32 grid of the padded image's pixel

@@ -1,4 +1,4 @@
-"""The C-ABI shared library builds for sm_100a, loads without a GPU and exports every symbol include/dvla.h declares."""
+"""The C-ABI shared library builds for sm_90a, loads without a GPU and exports every symbol include/dvla.h declares."""
 import ctypes
 import os
 import re
@@ -43,13 +43,14 @@ def test_invalid_args_return_error_not_abort(lib_path):
     assert b"null" in lib.dvla_last_error()
 
 
-def test_sass_is_blackwell_native(lib_path):
-    """tcgen05.mma / TMA / TMEM loads must be present in the SASS of the shipped library (UTCHMMA, UTMALDG, LDTM)."""
+def test_sass_is_hopper_native(lib_path):
+    """wgmma / TMA / mbarrier transaction waits must be present in the SASS of the shipped library (HGMMA, UTMALDG, SYNCS)."""
     try:
         sass = subprocess.run(["cuobjdump", "-sass", lib_path], capture_output=True, text=True, timeout=300).stdout
     except FileNotFoundError:
         pytest.skip("cuobjdump not available")
-    for mnemonic in ("UTCHMMA", "UTMALDG", "LDTM"):
+    assert "arch = sm_90a" in sass
+    for mnemonic in ("HGMMA.64x128x16.F32.BF16", "UTMALDG", "SYNCS.PHASECHK.TRANS64"):
         assert mnemonic in sass, f"{mnemonic} missing from SASS"
 
 

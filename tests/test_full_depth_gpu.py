@@ -11,14 +11,12 @@ and against the fp32 oracle run on the same GPU (oracle/, pinned to those golden
 The bar (SURVEY §7, VERDICT r1 item 1b): err_ours <= err_ref_bf16 + 1e-3 -- "no worse than the reference's own bf16 path".
 It is asserted strictly on the MEAN over all compared tensors, and per tensor with a band of 5 % of the reference's own
 error on top: the weight-gradient GEMMs add their split-K partial sums with atomics, so this package's error moves by up to
-~7e-4 from run to run (measured over three B200 runs: every tensor inside the strict bound in one run, two of ~78 outside it
-by <= 5.3e-4 in the others).  All achieved errors, the strict margins and the number of strict misses are printed.
+~7e-4 from run to run (so some tensors may miss the strict bound by a few 1e-4 in a given run).  All achieved errors, the strict margins and the number of strict misses are printed.
 
 SCALAR quantities (a loss value) are one draw of the rounding noise, not an average over a tensor, and the draw is
-dominated by a few shared upstream roundings (correlated across the loss's elements): across the B200 runs of this repo the
-relative error of the same loss moved between 3.9e-4 and 2.4e-3 for this package and between 4.4e-4 and 2.8e-3 for the
-reference-style bf16 run, from one kernel revision / configuration to the next, while every gradient tensor stayed inside
-its bound.  For scalars the bound is therefore max(err_ref_bf16 + 1e-3, 2^-8): an error below half a bf16 ulp of the value
+dominated by a few shared upstream roundings (correlated across the loss's elements): the relative
+error of the same loss moves by several 1e-4 from one kernel revision / configuration to the next, for this package and
+for the reference-style bf16 run alike, while every gradient tensor stays inside its bound.  For scalars the bound is therefore max(err_ref_bf16 + 1e-3, 2^-8): an error below half a bf16 ulp of the value
 itself is below the resolution of every activation that feeds it.  The strict comparison is still printed.
 """
 import json

@@ -1,6 +1,6 @@
 """Host logic of the GEMM dispatcher, without a GPU: `dvla_gemm_plan` runs the same code as `dvla_gemm` up to the point where
 tensor maps would be encoded and the kernel launched, and `dvla_gemm_plan_unit` evaluates the same unit -> (tile, k-range)
-map the persistent kernels walk (`map_unit`, shared host/device function in csrc/gemm_sm100.cu).
+map the persistent kernels walk (`map_unit`, shared host/device function in csrc/gemm_sm90.cu).
 
 Checked over the GEMM shapes of the C2 / C3 / C4 workloads, their weight-gradient forms, and a random sweep:
   * every (output tile, k-block) is covered by exactly one work unit -- whole tiles, uniform split-K and the K-split tail;
@@ -58,7 +58,7 @@ def units(lib, p):
 
 def check_cover(lib, p, M, N, K):
     """Every k-block of every tile exactly once; returns the unit list."""
-    assert p.kernel in (2, 3)
+    assert p.kernel == 2
     assert p.m_tiles == -(-M // p.tile_m) and p.n_tiles == -(-N // p.tile_n) and p.k_blocks == -(-K // 64)
     tiles = p.m_tiles * p.n_tiles
     seen = [[0] * p.k_blocks for _ in range(tiles)]
@@ -71,7 +71,7 @@ def check_cover(lib, p, M, N, K):
     return us
 
 
-def check_tail(lib, p, us, slots_per_wave, ctas_per_tile):
+def check_tail(lib, p, us, slots_per_wave):
     tiles = p.m_tiles * p.n_tiles
     if p.tail_splits <= 1:
         assert all(slot < 0 for (_, _, _, slot, _) in us)
@@ -85,10 +85,9 @@ def check_tail(lib, p, us, slots_per_wave, ctas_per_tile):
             assert (t, k0, k1, slot) == (u, 0, p.k_blocks, -1)
         else:
             assert slot == t - p.tail_first and 0 <= split < p.tail_splits and k0 == split * p.tail_kbps
-    # workspace: 64 KB of counters (16 per CTA slot) + one fp32 slice of 128 x tile_n(CTA) per CTA slot and split
-    cta_cols = 256 if p.kernel == 3 else p.tile_n
-    need = 65536 + n_tail * ctas_per_tile * p.tail_splits * 128 * cta_cols * 4
-    assert need <= int(lib.dvla_gemm_workspace_bytes(None)) and n_tail * ctas_per_tile * 16 * 4 <= 65536
+    # workspace: 64 KB of counters (8 per CTA slot) + one fp32 slice of 128 x tile_n per CTA slot and split
+    need = 65536 + n_tail * p.tail_splits * 128 * p.tile_n * 4
+    assert need <= int(lib.dvla_gemm_workspace_bytes(None)) and n_tail * 8 * 4 <= 65536
 
 
 WORKLOAD = [  # (M, N, K, b_mn)  forward / dgrad GEMMs of C2 at B=8 and B=2, C3 at B=16, C4 (action inference)
@@ -101,19 +100,17 @@ WORKLOAD = [  # (M, N, K, b_mn)  forward / dgrad GEMMs of C2 at B=8 and B=2, C3 
 ]
 
 
-@pytest.mark.parametrize("sms", [148, 132])
+@pytest.mark.parametrize("sms", [132, 116])
 def test_workload_gemms_are_covered_exactly_once(lib, sms):
     lib.dvla_set_sm_budget(sms)
     try:
         for (M, N, K, b_mn) in WORKLOAD:
             p = plan(lib, M, N, K, b_mn=b_mn, bias=True)
             us = check_cover(lib, p, M, N, K)
-            pair = p.kernel == 3
-            slots = sms // 2 if pair else sms
-            check_tail(lib, p, us, slots, 2 if pair else 1)
+            check_tail(lib, p, us, sms)
             assert p.grid_ctas <= sms and p.k_splits == 1 and not p.atomic_out, "a GEMM with an epilogue never splits K uniformly"
             tiles = p.m_tiles * p.n_tiles
-            if tiles < slots:
+            if tiles < sms:
                 assert p.tail_splits <= 1, "sub-wave GEMMs keep one K order whatever the batch (batch invariance)"
     finally:
         lib.dvla_set_sm_budget(0)
@@ -121,13 +118,13 @@ def test_workload_gemms_are_covered_exactly_once(lib, sms):
 
 def test_known_decisions(lib):
     lib.dvla_set_sm_budget(0)
-    p = plan(lib, 10320, 1024, 4096, b_mn=True, bias=True)          # 41 x 4 = 164 pair tiles on 74 pairs: 2 waves + 16
-    assert (p.kernel, p.tile_m, p.tile_n, p.tail_first, p.tail_splits, p.tail_kbps) == (3, 256, 256, 148, 4, 16)
-    assert p.units == 148 + 16 * 4 and p.grid_ctas == 148
-    p = plan(lib, 10320, 1024, 1024, b_mn=True, bias=True)          # 16 k-blocks: the fix-up would cost more than the wave
+    p = plan(lib, 2580, 1024, 4096, b_mn=True, bias=True)           # 21 x 8 = 168 tiles on 132 SMs: 1 wave + 36
+    assert (p.kernel, p.tile_m, p.tile_n, p.tail_first, p.tail_splits, p.tail_kbps) == (2, 128, 128, 132, 3, 22)
+    assert p.units == 132 + 36 * 3 and p.grid_ctas == 132
+    p = plan(lib, 2580, 1024, 1024, b_mn=True, bias=True)           # 16 k-blocks: the fix-up would cost more than the wave
     assert p.tail_splits <= 1
-    p = plan(lib, 10320, 1024, 4096, b_mn=True, bias=True, workspace=False)
-    assert p.tail_splits <= 1 and p.units == 164
+    p = plan(lib, 2580, 1024, 4096, b_mn=True, bias=True, workspace=False)
+    assert p.tail_splits <= 1 and p.units == 168
     p = plan(lib, 21, 7, 768, bias=True, ldb=768)                   # N = 7: TMA-addressable operands but a 7-wide output
     assert p.kernel in (0, 1, 2)
     p = plan(lib, 21, 768, 6, lda=6, ldb=6)                         # K = 6: rows are not 16-byte multiples -> SIMT kernel
@@ -147,7 +144,7 @@ def test_weight_gradient_split_k(lib):
         elif p.k_splits > 1:
             assert p.atomic_out == 1 and p.kb_per_split * p.k_splits >= p.k_blocks > p.kb_per_split * (p.k_splits - 1)
         tiles = p.m_tiles * p.n_tiles
-        slots = 74 if p.kernel == 3 else 148
+        slots = 132
         if K >= 10320 and tiles * 2 <= slots:
             assert max(p.k_splits, p.tail_splits) > 1, "a long contraction over a few tiles must be split"
 
@@ -166,6 +163,5 @@ def test_random_shapes(lib):
             continue
         us = check_cover(lib, p, M, N, K)
         if not accumulate:
-            pair = p.kernel == 3
-            check_tail(lib, p, us, 74 if pair else 148, 2 if pair else 1)
+            check_tail(lib, p, us, 132)
             assert p.k_splits == 1

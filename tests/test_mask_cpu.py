@@ -1,5 +1,5 @@
 """Bit-exact contract for the attention mask (dreamvla_model.py:25-66): product generator == oracle generator ==
-reference generator (when present) == golden packed mask, for every flag combination the shipped scripts use."""
+reference generator (its masks' digests in tests/golden/reference_checks.pt) == golden packed mask, for every flag combination the shipped scripts use."""
 import itertools
 import json
 import os
@@ -10,9 +10,9 @@ import torch
 
 from dreamvla_b200.models.dreamvla_model import generate_attention_mask as gen_product
 from dreamvla_b200.ops import AttnMask
-from oracle import ref_shims
 from oracle.dreamvla_oracle import generate_attention_mask as gen_oracle
 from tests import synth
+from tests.digests import digest
 
 GOLDEN = os.path.join(os.path.dirname(__file__), "golden")
 COMBOS = [dict(K=K, num_A=36, num_B=nobs + 3, atten_goal=ag, atten_goal_state=ags, atten_only_obs=aoo,
@@ -30,16 +30,13 @@ def test_product_equals_oracle(kw):
     assert torch.equal(a, b)
 
 
-@pytest.mark.skipif(not ref_shims.reference_available(), reason="reference tree not present")
 @pytest.mark.parametrize("kw", COMBOS[::7])
 def test_product_equals_reference(kw):
-    ref_shims.install()
-    from models.dreamvla_model import generate_attention_mask as gen_ref
     np.random.seed(5)
     a = gen_product(**kw)
-    np.random.seed(5)
-    b = gen_ref(**kw)
-    assert torch.equal(a, b)
+    ref = torch.load(os.path.join(GOLDEN, "reference_checks.pt"))["mask"][COMBOS[::7].index(kw)]
+    assert ref["kw"] == kw
+    assert digest(a) == ref["digest"], "mask differs from the reference generator's"
 
 
 @pytest.mark.parametrize("name", list(synth.CASES))

@@ -88,7 +88,7 @@ def test_incremental_rollout_matches_full_window(dev, case, prune):
     prune=False feeds the backbone the same L tokens as the full window: the selected rows see identical inputs, so the
     actions agree to the last bit of the fp16 action the wrapper returns.
     prune=True drops never-attended tokens: the same mathematics on another sequence length, i.e. other flash-attention
-    tiles (or another kernel: L = 39 takes the mma.sync path, L = 117 the tcgen05 one).  The backbone's action-token rows
+    tiles.  The backbone's action-token rows
     -- the quantity the pruning touches -- agree to bf16 rounding; the 10-step guided sampler on top of random synthetic
     weights amplifies that, so the actions get a wide bar (a trained model's sampler is far better conditioned)."""
     from dreamvla_b200.utils.eval_utils_calvin import ModelWrapper

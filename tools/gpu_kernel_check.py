@@ -1,6 +1,6 @@
-"""Diagnostic sweep of every kernel in libdvla_sm100.so against plain PyTorch fp32 references ON THE GPU.
+"""Diagnostic sweep of every kernel in libdvla_sm90.so against plain PyTorch fp32 references ON THE GPU.
 
-Usage (on a B200 box):  python tools/gpu_kernel_check.py <group> [--json out.json]
+Usage (on an H100):  python tools/gpu_kernel_check.py <group> [--json out.json]
 Groups run in separate processes (a trapped kernel poisons its CUDA context).  This is a development tool;
 the graded parity tests are tests/test_*_gpu.py.
 """
@@ -281,7 +281,7 @@ def attn_case(B, H, Lq, Lk, masked, fused_qkv=False, seed=3, timeit=False, ramp=
         if ramp:      # key norms grow along the sequence: the running row max keeps rising (online-softmax rescale path)
             k = (k.float() * (1.0 + ramp * torch.arange(Lk, device=dev).view(1, Lk, 1, 1) / Lk)).to(torch.bfloat16)
             q = (q.float() * 2.0).to(torch.bfloat16)
-    mask_bool = bits = flags = bits_t = None
+    mask_bool = bits = flags = None
     if masked:
         mask_bool = torch.rand(Lq, Lk, generator=g) < 0.3
         mask_bool[:, 0] = True                       # no fully-masked rows
@@ -289,7 +289,6 @@ def attn_case(B, H, Lq, Lk, masked, fused_qkv=False, seed=3, timeit=False, ramp=
             mask_bool[: Lq // 2, 64:128] = False     # a fully masked tile
             mask_bool[Lq // 2:, 64:128] = True       # a fully visible one (if Lq//2 is tile aligned)
         bits = pack_mask(mask_bool)
-        bits_t = pack_mask(mask_bool.t().contiguous())
         flags = L.attn_mask_tiles(bits, Lq, Lk)
         mask_bool = mask_bool.to(dev)
     scale = 0.125
@@ -308,10 +307,10 @@ def attn_case(B, H, Lq, Lk, masked, fused_qkv=False, seed=3, timeit=False, ramp=
         dq, dk, dv = dqkv[:, :, 0], dqkv[:, :, 1], dqkv[:, :, 2]
     else:
         dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
-    L.attn_bwd(q, k, v, o, d_o, lse, scale, dq, dk, dv, bits, flags, mask_bits_t=bits_t)
+    L.attn_bwd(q, k, v, o, d_o, lse, scale, dq, dk, dv, bits, flags)
     oref.backward(d_o.float())
     if timeit:
-        ms = bench(lambda: L.attn_bwd(q, k, v, o, d_o, lse, scale, dq, dk, dv, bits, flags, mask_bits_t=bits_t))
+        ms = bench(lambda: L.attn_bwd(q, k, v, o, d_o, lse, scale, dq, dk, dv, bits, flags))
         extra = f"bwd {ms*1e3:.1f}us"
     report(tag + " dq", rel(dq, qr.grad), 1e-2, extra)
     report(tag + " dk", rel(dk, kr.grad), 1e-2)
@@ -402,15 +401,15 @@ def group_attn_perf():
     def run(tag, B, H, L, mask=None, p=0.0):
         qkv = torch.randn(B, L, 3, H, 64, generator=g).to(dev, torch.bfloat16)
         q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
-        bits = flags = bits_t = None
+        bits = flags = None
         if mask is not None:
-            bits, bits_t, flags = mask.bits, mask.bits_t, mask.flags
+            bits, flags = mask.bits, mask.flags
         o, lse = L_.attn_fwd(q, k, v, 0.125, bits, flags, dropout_p=p, dropout_seed=5)
         d_o = torch.randn(B, L, H, 64, generator=g).to(dev, torch.bfloat16)
         dqkv = torch.empty_like(qkv)
         f = bench(lambda: L_.attn_fwd(q, k, v, 0.125, bits, flags, dropout_p=p, dropout_seed=5))
         bw = bench(lambda: L_.attn_bwd(q, k, v, o, d_o, lse, 0.125, dqkv[:, :, 0], dqkv[:, :, 1], dqkv[:, :, 2], bits, flags,
-                                       mask_bits_t=bits_t, dropout_p=p, dropout_seed=5))
+                                       dropout_p=p, dropout_seed=5))
         vis = float(L * L) if mask is None else float(mask.visible)
         gf = 4 * 64 * vis * B * H / 1e9
         print(f"INFO attn_perf {tag:28s} fwd {f*1e3:7.1f} us ({gf/f:6.0f} TF/s)  bwd {bw*1e3:7.1f} us ({2.5*gf/bw:6.0f} TF/s)", flush=True)
@@ -454,9 +453,9 @@ def group_attn_perf():
 
         def bwd():
             L_.attn_bwd(q[:, :n_main], k[:, :n_ka], v[:, :n_ka], o1, d_o[:, :n_main], l1, 0.125, dqkv[:, :n_main, 0], dqkv[:, :n_ka, 1],
-                        dqkv[:, :n_ka, 2], am_main.bits, am_main.flags, mask_bits_t=am_main.bits_t, dropout_p=p_drop, dropout_seed=5)
+                        dqkv[:, :n_ka, 2], am_main.bits, am_main.flags, dropout_p=p_drop, dropout_seed=5)
             L_.attn_bwd(q[:, n_main:], k[:, :n_main], v[:, :n_main], o2, d_o[:, n_main:], l2, 0.125, dqkv[:, n_main:, 0], dk_act, dv_act,
-                        am_act.bits, am_act.flags, mask_bits_t=am_act.bits_t, dropout_p=p_drop, dropout_seed=6)
+                        am_act.bits, am_act.flags, dropout_p=p_drop, dropout_seed=6)
         f, bw = bench(fwd), bench(bwd)
         print(f"INFO attn_perf gpt2 GROUPED main 1260x360 + act 30x1260, drop={p_drop}: fwd {f*1e3:7.1f} us  bwd {bw*1e3:7.1f} us", flush=True)
     report("attn_perf ran", 0.0, 1.0)

@@ -1,6 +1,6 @@
 """Summarise an `ncu --set full` report (.ncu-rep) per kernel launch: duration, occupancy limiters, pipe utilisation
 (tensor, XU/MUFU, FMA), issue-slot utilisation, DRAM / L2 throughput, top warp-stall reasons.
-usage: python tools/ncu_kernel_summary.py report.ncu-rep > profiles/xyz.txt"""
+usage: python tools/ncu_kernel_summary.py report.ncu-rep > summary.txt"""
 import csv
 import subprocess
 import sys

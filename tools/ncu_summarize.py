@@ -16,7 +16,7 @@ for r in rd:
         continue
     name = r["Kernel Name"]
     name = re.sub(r"\(.*$", "", name)
-    name = re.sub(r"<.*$", "", name) if not name.startswith("dvla::gemm") and "gemm_tcgen05" not in name else name
+    name = re.sub(r"<.*$", "", name) if not name.startswith("dvla::gemm") and "gemm_wgmma" not in name else name
     v = float(r["Metric Value"].replace(",", ""))
     unit = r.get("Metric Unit", "ns")
     if unit in ("us", "usecond"):

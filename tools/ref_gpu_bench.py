@@ -1,7 +1,7 @@
 """Context number, NOT a bench arm: the reference's algorithm (oracle/, a functional PyTorch restatement) run on the GPU
 the way the reference itself runs (PyTorch eager kernels + cuBLAS under torch.autocast(bf16), fp32 master weights,
 torch.optim.AdamW, clip_grad_norm_) — BASELINE.md §3 "reference GPU build".  Prints one JSON line per batch size so that
-profiles/ can quote  ours / (stock PyTorch)  on the same B200.  Test/measurement infrastructure: imports oracle/.
+a result can quote  ours / (stock PyTorch)  on the same GPU.  Test/measurement infrastructure: imports oracle/.
 
   python tools/ref_gpu_bench.py [--batch 2 8] [--sdpa] [--steps 5]
 """

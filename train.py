@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Entry point mirroring reference train.py:40-297 for the B200-native hot path.
+"""Entry point mirroring reference train.py:40-297 for the H100-native hot path.
 
   torchrun --nnodes=1 --nproc_per_node=8 train.py <reference flags ...> [--synthetic_steps N] [--cuda_graph]
 
