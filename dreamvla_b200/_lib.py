@@ -72,6 +72,12 @@ class AdamWArgs(C.Structure):
                 ("max_norm", _f32), ("grad_scale", _f32), ("zero_grad", _i32)]
 
 
+class AdamWMasterArgs(C.Structure):
+    _fields_ = [("p32", _vp), ("p", _vp), ("g", _vp), ("m", _vp), ("v", _vp), ("n", _i64), ("sumsq", _vp), ("lr", _vp),
+                ("step", _vp), ("beta1", _f32), ("beta2", _f32), ("eps", _f32), ("weight_decay", _f32),
+                ("max_norm", _f32), ("grad_scale", _f32), ("zero_grad", _i32)]
+
+
 class DitBlockWeights(C.Structure):
     _fields_ = [(n, _vp) for n in ("qkv_w", "qkv_b", "proj_w", "proj_b", "fc1_w", "fc1_b", "fc2_w", "fc2_b")]
 
@@ -90,7 +96,7 @@ EXPORTS = [
     "dvla_version", "dvla_last_error", "dvla_launch_count", "dvla_gemm", "dvla_gemm_plan", "dvla_gemm_plan_unit", "dvla_layernorm_fwd", "dvla_layernorm_bwd",
     "dvla_attn_fwd", "dvla_attn_bwd", "dvla_attn_mask_tiles", "dvla_colsum_accum", "dvla_accum_fp32_into_bf16",
     "dvla_dropout", "dvla_act_bwd", "dvla_act_bwd_colsum", "dvla_cat_broadcast", "dvla_shift_crop", "dvla_resize_nearest", "dvla_mse_loss", "dvla_cosine_loss", "dvla_silog_stats", "dvla_silog_finish",
-    "dvla_sumsq", "dvla_adamw", "dvla_grad_clip_scale", "dvla_attn_bwd_workspace_bytes", "dvla_silog_workspace_bytes",
+    "dvla_sumsq", "dvla_adamw", "dvla_adamw_master", "dvla_grad_clip_scale", "dvla_attn_bwd_workspace_bytes", "dvla_silog_workspace_bytes",
     "dvla_gemm_workspace_bytes", "dvla_set_sm_budget", "dvla_dit_ddim_sample", "dvla_dit_sampler_workspace_bytes",
 ]
 
@@ -401,6 +407,17 @@ def adamw(p, g, m, v, *, sumsq_t, lr_t, step_t, beta1, beta2, eps, weight_decay,
     a = AdamWArgs(p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), p.numel(), _ptr(sumsq_t), lr_t.data_ptr(),
                   step_t.data_ptr(), beta1, beta2, eps, weight_decay, max_norm, grad_scale, int(zero_grad))
     _check(load().dvla_adamw(C.byref(a), _stream()), "dvla_adamw")
+
+
+def adamw_master(p32, p, g, m, v, *, sumsq_t, lr_t, step_t, beta1, beta2, eps, weight_decay, max_norm, grad_scale=1.0,
+                 zero_grad=True):
+    """`adamw` on fp32 master weights `p32`; the bf16 working copy `p` is overwritten with p32 rounded to bf16."""
+    _need_cuda(p32, p, g, m, v)
+    assert p32.dtype == torch.float32 and p.dtype == torch.bfloat16 and p32.numel() == p.numel() == g.numel() == m.numel()
+    a = AdamWMasterArgs(p32.data_ptr(), p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), p32.numel(), _ptr(sumsq_t),
+                        lr_t.data_ptr(), step_t.data_ptr(), beta1, beta2, eps, weight_decay, max_norm, grad_scale,
+                        int(zero_grad))
+    _check(load().dvla_adamw_master(C.byref(a), _stream()), "dvla_adamw_master")
 
 
 def grad_clip_scale(g, sumsq_t, max_norm, grad_scale=1.0):

@@ -66,6 +66,7 @@ int silog_finish_dispatch(const void* pred, const void* label, int64_t n, const 
                           float* loss_out, void* dpred, cudaStream_t s);
 int sumsq_dispatch(const void* g, int64_t n, float* out, cudaStream_t s);
 int adamw_dispatch(const dvla_adamw_args* a, cudaStream_t s);
+int adamw_master_dispatch(const dvla_adamw_master_args* a, cudaStream_t s);
 int grad_clip_scale_dispatch(void* g, int64_t n, const float* sumsq, float max_norm, float grad_scale, cudaStream_t s);
 
 }  // namespace dvla
@@ -138,6 +139,7 @@ int dvla_silog_finish(const void* pred, const void* label, int64_t n, const floa
 }
 int dvla_sumsq(const void* g, int64_t n, float* out, void* stream) { return sumsq_dispatch(g, n, out, S(stream)); }
 int dvla_adamw(const dvla_adamw_args* a, void* stream) { return adamw_dispatch(a, S(stream)); }
+int dvla_adamw_master(const dvla_adamw_master_args* a, void* stream) { return adamw_master_dispatch(a, S(stream)); }
 int dvla_grad_clip_scale(void* g, int64_t n, const float* sumsq, float max_norm, float grad_scale, void* stream) {
   return grad_clip_scale_dispatch(g, n, sumsq, max_norm, grad_scale, S(stream));
 }

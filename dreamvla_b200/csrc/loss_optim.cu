@@ -316,4 +316,89 @@ int adamw_dispatch(const dvla_adamw_args* a, cudaStream_t s) {
   return DVLA_OK;
 }
 
+// The same clip + AdamW on fp32 master weights: the update lands in p32 (no bf16 rounding of the parameter between
+// steps), then the bf16 working copy the kernels read is written as round-to-nearest(p32).  Same formula and operation
+// order as adamw_kernel, except that the decay product p * (1 - lr*wd) is rounded on its own (__fmul_rn, no FMA with the
+// update), as torch.optim.AdamW's `param.mul_(1 - lr * wd)` does: at lr*wd ~ 1e-7 the decay is about one fp32 ulp of the
+// weight, and folding its rounding into the update's drifts the fp32 trajectory by ~6e-4 of the accumulated update over
+// 100 steps (2.5e-6 with the separate rounding).  The old bf16 copy is never read.  30 B per parameter (adamw_kernel: 24).
+struct AdamWMasterParams {
+  float* p32; bf16* p; bf16* g; float* m; float* v; long long n;
+  const float* sumsq; const float* lr; const float* step;
+  float beta1, beta2, eps, wd, max_norm, grad_scale; int zero_grad;
+};
+__global__ void __launch_bounds__(256) adamw_master_kernel(AdamWMasterParams a) {
+  float clip = a.grad_scale;
+  if (a.sumsq) {
+    const float norm = sqrtf(a.sumsq[0]) * a.grad_scale;
+    clip *= fminf(1.0f, a.max_norm / (norm + 1e-6f));  // torch.nn.utils.clip_grad_norm_ semantics
+  }
+  const float lr = a.lr[0];
+  const float t = a.step[0];
+  const float bc1 = 1.0f - powf(a.beta1, t);
+  const float bc2s = sqrtf(1.0f - powf(a.beta2, t));
+  const float step_size = lr / bc1;
+  const float decay = 1.0f - lr * a.wd;
+  const long long nv = a.n >> 3;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < nv;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const uint4 gu = reinterpret_cast<const uint4*>(a.g)[i];
+    float4 p0 = reinterpret_cast<float4*>(a.p32)[2 * i], p1 = reinterpret_cast<float4*>(a.p32)[2 * i + 1];
+    float4 m0 = reinterpret_cast<float4*>(a.m)[2 * i], m1 = reinterpret_cast<float4*>(a.m)[2 * i + 1];
+    float4 v0 = reinterpret_cast<float4*>(a.v)[2 * i], v1 = reinterpret_cast<float4*>(a.v)[2 * i + 1];
+    float pf[8] = {p0.x, p0.y, p0.z, p0.w, p1.x, p1.y, p1.z, p1.w}, gf[8],
+          mf[8] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w}, vf[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
+    float2 f;
+    f = unpack_bf16x2(gu.x); gf[0] = f.x; gf[1] = f.y; f = unpack_bf16x2(gu.y); gf[2] = f.x; gf[3] = f.y;
+    f = unpack_bf16x2(gu.z); gf[4] = f.x; gf[5] = f.y; f = unpack_bf16x2(gu.w); gf[6] = f.x; gf[7] = f.y;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float gj = gf[j] * clip;
+      mf[j] = a.beta1 * mf[j] + (1.0f - a.beta1) * gj;
+      vf[j] = a.beta2 * vf[j] + (1.0f - a.beta2) * gj * gj;
+      const float denom = sqrtf(vf[j]) / bc2s + a.eps;
+      pf[j] = __fmul_rn(pf[j], decay) - step_size * mf[j] / denom;
+    }
+    reinterpret_cast<float4*>(a.p32)[2 * i] = make_float4(pf[0], pf[1], pf[2], pf[3]);
+    reinterpret_cast<float4*>(a.p32)[2 * i + 1] = make_float4(pf[4], pf[5], pf[6], pf[7]);
+    reinterpret_cast<uint4*>(a.p)[i] =
+        make_uint4(pack_bf16x2(pf[0], pf[1]), pack_bf16x2(pf[2], pf[3]), pack_bf16x2(pf[4], pf[5]), pack_bf16x2(pf[6], pf[7]));
+    reinterpret_cast<float4*>(a.m)[2 * i] = make_float4(mf[0], mf[1], mf[2], mf[3]);
+    reinterpret_cast<float4*>(a.m)[2 * i + 1] = make_float4(mf[4], mf[5], mf[6], mf[7]);
+    reinterpret_cast<float4*>(a.v)[2 * i] = make_float4(vf[0], vf[1], vf[2], vf[3]);
+    reinterpret_cast<float4*>(a.v)[2 * i + 1] = make_float4(vf[4], vf[5], vf[6], vf[7]);
+    if (a.zero_grad) reinterpret_cast<uint4*>(a.g)[i] = make_uint4(0, 0, 0, 0);
+  }
+  if (blockIdx.x == 0) {
+    for (long long i = (nv << 3) + threadIdx.x; i < a.n; i += blockDim.x) {
+      const float gj = __bfloat162float(a.g[i]) * clip;
+      const float mj = a.beta1 * a.m[i] + (1.0f - a.beta1) * gj;
+      const float vj = a.beta2 * a.v[i] + (1.0f - a.beta2) * gj * gj;
+      a.m[i] = mj; a.v[i] = vj;
+      const float denom = sqrtf(vj) / bc2s + a.eps;
+      const float pj = __fmul_rn(a.p32[i], decay) - step_size * mj / denom;
+      a.p32[i] = pj;
+      a.p[i] = __float2bfloat16_rn(pj);
+      if (a.zero_grad) a.g[i] = __float2bfloat16(0.f);
+    }
+  }
+}
+int adamw_master_dispatch(const dvla_adamw_master_args* a, cudaStream_t s) {
+  if (!a || !a->p32 || !a->p || !a->g || !a->m || !a->v || !a->lr || !a->step) {
+    set_error("adamw_master: null pointer");
+    return DVLA_ERR_INVALID;
+  }
+  if ((reinterpret_cast<uintptr_t>(a->p32) | reinterpret_cast<uintptr_t>(a->p) | reinterpret_cast<uintptr_t>(a->g) |
+       reinterpret_cast<uintptr_t>(a->m) | reinterpret_cast<uintptr_t>(a->v)) & 15) {
+    set_error("adamw_master: buffers must be 16-byte aligned");
+    return DVLA_ERR_INVALID;
+  }
+  if (a->n <= 0) return DVLA_OK;
+  AdamWMasterParams k{a->p32, (bf16*)a->p, (bf16*)a->g, a->m, a->v, a->n, a->sumsq, a->lr, a->step,
+                      a->beta1, a->beta2, a->eps, a->weight_decay, a->max_norm, a->grad_scale, a->zero_grad};
+  adamw_master_kernel<<<grid_for(a->n, 256 * 8 * 2), 256, 0, s>>>(k);
+  DVLA_CHECK_LAUNCH("adamw_master");
+  return DVLA_OK;
+}
+
 }  // namespace dvla

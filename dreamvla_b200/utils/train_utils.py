@@ -10,8 +10,8 @@ Here:
   * losses are fused value+gradient kernels (ops.mse_loss / cosine_loss / silog_loss), no host sync in the step;
   * data-parallel: the flat bf16 gradient buffer is laid out in order of backward completion and all-reduced (NCCL over
     NVLink, communication stream) in three segments, the first two from backward hooks while backward continues; then
-    an order-deterministic global norm + clip + AdamW in two kernels (dvla_sumsq, dvla_adamw); lr / step counters live
-    on the device;
+    an order-deterministic global norm + clip + AdamW in two kernels (dvla_sumsq, dvla_adamw; dvla_adamw_master on fp32
+    master weights under --precision fp32); lr / step counters live on the device;
   * the per-step `.cpu().numpy()` visual-debug copies of the reference (:198-213, :382-396) are not part of the path.
 """
 from __future__ import annotations
@@ -190,9 +190,13 @@ class FlatParams:
 
     Layout: [ >=2-D parameters | 1-D parameters ], each parameter 16-byte aligned.  Parameters become views of `P`;
     `p.grad` is a view of `G`; ops accumulate weight gradients through `p._dvla_grad` and 1-D gradients in fp32
-    through `p._dvla_grad32` (folded into G by `fold_small_grads`)."""
+    through `p._dvla_grad32` (folded into G by `fold_small_grads`).
 
-    def __init__(self, model, cfg: StepConfig, exclude_prefixes=()):
+    `master` (`--precision fp32`): a dict name -> fp32 tensor with the fp32 values of (at least) the trainable parameters.
+    Then `P32` holds fp32 master weights in the same layout as `P`, AdamW updates `P32` (dvla_adamw_master) and `P` is
+    the bf16 working copy, rounded from `P32` once per optimiser step.  Without it `P32` is None and AdamW updates `P`."""
+
+    def __init__(self, model, cfg: StepConfig, exclude_prefixes=(), master=None):
         inactive = []
         for head, on in (("image", cfg.loss_image), ("depth", cfg.loss_depth), ("dino", cfg.loss_dino_feat),
                          ("sam", cfg.loss_sam_feat), ("traj", cfg.loss_trajectory)):
@@ -236,9 +240,18 @@ class FlatParams:
         self.sumsq = torch.zeros(1, device=dev, dtype=torch.float32)
         self.lr = torch.zeros(1, device=dev, dtype=torch.float32)
         self.step_count = torch.zeros(1, device=dev, dtype=torch.float32)
+        self.P32 = None
+        if master is not None:
+            self.P32 = torch.zeros(self.n, device=dev, dtype=torch.float32)
+            for (name, p), o in zip(self.params, offs):
+                if name not in master or master[name].shape != p.shape:
+                    raise RuntimeError(f"FlatParams: no fp32 master value of shape {tuple(p.shape)} for {name}")
+                self.P32[o:o + p.numel()].copy_(master[name].reshape(-1))
+            self.P.copy_(self.P32)
         for (name, p), o in zip(self.params, offs):
             n = p.numel()
-            self.P[o:o + n].copy_(p.data.reshape(-1))
+            if self.P32 is None:
+                self.P[o:o + n].copy_(p.data.reshape(-1))
             p.data = self.P[o:o + n].view(p.shape)
             g = self.G[o:o + n].view(p.shape)
             p.grad = g
@@ -246,7 +259,21 @@ class FlatParams:
             if p.dim() <= 1:
                 p._dvla_grad32 = self.G32[o - self.n_big:o - self.n_big + n]
             self.names.append(name)
+        self.offsets = offs
         self.num_params = sum(p.numel() for _, p in self.params)
+        # fp32 values of the trainable parameters this step never updates (NEVER_USED_PREFIXES, heads whose loss is off),
+        # kept on the host so that a checkpoint writes back exactly what was loaded
+        trained = set(self.names)
+        self.master_rest = {} if master is None else {
+            name: master[name].detach().to("cpu", torch.float32).clone() for name, p in model.named_parameters()
+            if p.requires_grad and name not in trained and name in master}
+
+    def master_state_dict(self):
+        """name -> fp32 value of every trainable parameter in fp32 mode: views of `P32` for the parameters the step trains,
+        then the host copies of `master_rest`."""
+        sd = {name: self.P32[o:o + p.numel()].view(p.shape) for (name, p), o in zip(self.params, self.offsets)}
+        sd.update(self.master_rest)
+        return sd
 
     def fold_small_grads(self):
         if self.n > self.n_big:
@@ -267,16 +294,20 @@ class FlatParams:
         if lr is not None:
             self.lr.fill_(lr)
         self.step_count += 1
+        if self.P32 is None:
+            def update(**kw):
+                L.adamw(self.P, self.G, self.m, self.v, **kw)
+        else:
+            def update(**kw):
+                L.adamw_master(self.P32, self.P, self.G, self.m, self.v, **kw)
         if preclipped:
-            L.adamw(self.P, self.G, self.m, self.v, sumsq_t=None, lr_t=self.lr, step_t=self.step_count, beta1=0.9,
-                    beta2=0.999, eps=1e-8, weight_decay=cfg.weight_decay, max_norm=cfg.max_grad_norm, grad_scale=1.0,
-                    zero_grad=True)
+            update(sumsq_t=None, lr_t=self.lr, step_t=self.step_count, beta1=0.9, beta2=0.999, eps=1e-8,
+                   weight_decay=cfg.weight_decay, max_norm=cfg.max_grad_norm, grad_scale=1.0, zero_grad=True)
             return
         self.sumsq.zero_()
         L.sumsq(self.G, self.sumsq)
-        L.adamw(self.P, self.G, self.m, self.v, sumsq_t=self.sumsq, lr_t=self.lr, step_t=self.step_count, beta1=0.9,
-                beta2=0.999, eps=1e-8, weight_decay=cfg.weight_decay, max_norm=cfg.max_grad_norm,
-                grad_scale=1.0 / world_size, zero_grad=True)
+        update(sumsq_t=self.sumsq, lr_t=self.lr, step_t=self.step_count, beta1=0.9, beta2=0.999, eps=1e-8,
+               weight_decay=cfg.weight_decay, max_norm=cfg.max_grad_norm, grad_scale=1.0 / world_size, zero_grad=True)
 
     def optimizer_state_dict(self):
         """AdamW state of the flat buffers.  NOT torch.optim.AdamW's format (the reference's `optimizer_state_dict`,
@@ -394,19 +425,24 @@ def all_reduce_flat(G, world_size, group=None, comm_stream=None):
 class TrainStep:
     """One micro-step of train_utils.py:94-608 on device-resident inputs; see module docstring."""
 
-    def __init__(self, model, cfg: StepConfig, world_size=1, process_group=None):
+    def __init__(self, model, cfg: StepConfig, world_size=1, process_group=None, master=None):
+        """`master`: fp32 values of the trainable parameters (name -> tensor) for fp32 master weights, see FlatParams."""
         if cfg.pred_num != 1:
             # the reference unfolds the labels over pred_num (train_utils.py:176-185); this step builds single-frame labels
             raise NotImplementedError("pred_num > 1 is not implemented in the train step (labels are not unfolded)")
         self.model, self.cfg = model, cfg
         self.world_size = world_size
         self.pg = process_group
-        self.flat = FlatParams(model, cfg)
+        self.flat = FlatParams(model, cfg, master=master)
         if world_size > 1:
             # DDP's constructor broadcasts rank 0's parameters and buffers (train.py:173); every replica must start from
             # the same weights or the shared all-reduced gradient is applied to different models
             import torch.distributed as dist
-            dist.broadcast(self.flat.P, src=0, group=process_group)
+            if self.flat.P32 is not None:
+                dist.broadcast(self.flat.P32, src=0, group=process_group)
+                self.flat.P.copy_(self.flat.P32)
+            else:
+                dist.broadcast(self.flat.P, src=0, group=process_group)
             for _, b in model.named_buffers():
                 if b.is_cuda:
                     dist.broadcast(b, src=0, group=process_group)

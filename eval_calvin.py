@@ -5,6 +5,8 @@ The CALVIN simulator (PyBullet) is out of scope; `--synthetic_rollout_steps N` d
 observations and reports p50 / p99 per-action latency (the latency metric of BASELINE.json).  A real env can call
 `dreamvla_b200.utils.eval_utils_calvin.ModelWrapper.step` exactly where the reference calls `model.step` (:264).
 `--incremental_rollout` switches the wrapper to rollout-level incremental inference (per-frame token cache, SURVEY §8 f-1).
+Inference runs in bf16 whatever `--precision` says: the fp32 checkpoints of a `--precision fp32` run (and the reference's)
+load by rounding each value to bf16.
 """
 from __future__ import annotations
 

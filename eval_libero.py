@@ -7,6 +7,7 @@ The LIBERO simulator (MuJoCo / robosuite) is out of scope; `--synthetic_rollout_
 `dreamvla_b200.utils.eval_utils_libero.ModelWrapper.step` with synthetic observations (agent-view and eye-in-hand images,
 end-effector position + quaternion, finger joint positions) and reports p50 / p99 per-action latency.  A real env calls
 `wrapper.step(...)` where the reference calls `model.step(obs, goal, steps)` (utils/eval_utils_libero.py:189).
+The model is bf16 (`eval_calvin.load_model`); fp32 checkpoints load by rounding each value to bf16.
 """
 from __future__ import annotations
 

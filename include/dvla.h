@@ -239,6 +239,23 @@ typedef struct {
   int32_t zero_grad;
 } dvla_adamw_args;
 int dvla_adamw(const dvla_adamw_args* args, void* stream);
+/* dvla_adamw_master: the same clip + AdamW (same formula, same operation order) on fp32 MASTER weights p32, for
+ * `--precision fp32`.  p32 is read and updated; the bf16 working copy p is written as round-to-nearest(p32) (exactly
+ * p32.to(torch.bfloat16)) and never read.  Gradients stay bf16.  30 B of HBM traffic per parameter (dvla_adamw: 24).
+ * All of p32, p, g, m, v 16-byte aligned. */
+typedef struct {
+  float* p32;         /* fp32 [n], read and written */
+  void* p;            /* bf16 [n], written only */
+  void* g;            /* bf16 [n] */
+  float* m; float* v; /* fp32 [n] */
+  int64_t n;
+  const float* sumsq; /* fp32 [1] or NULL (gradient already clipped) */
+  const float* lr;    /* fp32 [1] device */
+  const float* step;  /* fp32 [1] device: step count AFTER increment (>= 1) */
+  float beta1, beta2, eps, weight_decay, max_norm, grad_scale;
+  int32_t zero_grad;
+} dvla_adamw_master_args;
+int dvla_adamw_master(const dvla_adamw_master_args* args, void* stream);
 /* In-place clip of the accumulated gradient, every micro-step, as utils/train_utils.py:599-600 does
  * (clip_grad_norm_ on .grad that keeps accumulating):  g *= grad_scale * min(1, max_norm / (sqrt(sumsq)*grad_scale + 1e-6)). */
 int dvla_grad_clip_scale(void* g_bf16, int64_t n, const float* sumsq, float max_norm, float grad_scale, void* stream);

@@ -526,6 +526,28 @@ def group_loss():
                 max_norm=0.1, zero_grad=True)
         assert Gw.abs().max().item() == 0
     report("adamw 3 steps (bf16 param rounding)", rel(Pc, pref.detach()), 8e-3)
+    # fp32 master weights: the same 3 steps on fp32 parameters, the bf16 working copy rounded from the master
+    P32 = P.float()
+    pref = P32.clone().requires_grad_(True)
+    opt = torch.optim.AdamW([pref], lr=1e-3, weight_decay=1e-2, betas=(0.9, 0.999), eps=1e-8)
+    m.zero_()
+    v.zero_()
+    step_t.zero_()
+    Pw = torch.empty_like(P)
+    for it in range(3):
+        Gi = (G.float() * (it + 1)).to(torch.bfloat16)
+        pref.grad = Gi.float().clone()
+        torch.nn.utils.clip_grad_norm_([pref], 0.1)
+        opt.step()
+        ss.zero_()
+        L.sumsq(Gi, ss)
+        step_t += 1
+        Gw = Gi.clone()
+        L.adamw_master(P32, Pw, Gw, m, v, sumsq_t=ss, lr_t=lr_t, step_t=step_t, beta1=0.9, beta2=0.999, eps=1e-8,
+                       weight_decay=1e-2, max_norm=0.1, zero_grad=True)
+        assert Gw.abs().max().item() == 0
+        assert torch.equal(Pw, P32.to(torch.bfloat16))
+    report("adamw_master 3 steps (fp32 update)", rel(P32 - P.float(), pref.detach() - P.float()), 1e-5)
     _check_sumsq_deterministic()
 
 

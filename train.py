@@ -3,8 +3,12 @@
 
   torchrun --nnodes=1 --nproc_per_node=8 train.py <reference flags ...> [--synthetic_steps N] [--cuda_graph]
 
-Builds `DreamVLA` from the reference's flags, casts to bf16 (`--precision bf16`; the kernels are bf16-only), sets up
-one process per GPU over NCCL, and runs `train_one_epoch_calvin` (dreamvla_b200/utils/train_utils.py).  Dataset loading
+Builds `DreamVLA` from the reference's flags, loads checkpoints into it in fp32, casts it to bf16 (the kernels are
+bf16-in / fp32-accumulate), sets up one process per GPU over NCCL, and runs `train_one_epoch_calvin`
+(dreamvla_b200/utils/train_utils.py).  `--precision fp32` (the reference's default) trains fp32 master weights: AdamW
+updates an fp32 copy of every trained parameter, the kernels read a bf16 copy rounded from it once per optimiser step, and
+checkpoints carry the fp32 values; `--bf16_module` may then name only the frozen `vision_encoder` / `text_encoder`, which
+run in bf16 anyway.  `--precision bf16` stores the parameters in bf16 only (see `resolve_precision`).  Dataset loading
 (utils/data_utils.py in the reference) is out of scope: pass `--synthetic_steps N` to train on the synthetic collator
 contract, or plug a loader that yields the reference's 13-tuple (data_utils.py:1395-1397) into `main(args, loader)`.
 Checkpoints keep the reference's layout (train.py:279-289): {"epoch", "model_state_dict" ("module."-prefixed, trainable
@@ -17,6 +21,7 @@ from __future__ import annotations
 import math
 import os
 import random
+import re
 
 import numpy as np
 import torch
@@ -129,27 +134,60 @@ class _ModuleWrapper:
         return (("module." + n, p) for n, p in self.module.named_parameters())
 
 
-def get_checkpoint(model):                  # train_utils.py:750-757
+def get_checkpoint(model, step=None):       # train_utils.py:750-757
+    """Trainable entries of `model.state_dict()`.  With the TrainStep of an fp32 run (`step.flat.P32` set) every trainable
+    parameter is written in fp32: the master weights, and the loaded fp32 value of parameters the step does not train."""
     sd = model.state_dict()
     for name, p in model.named_parameters():
         if name in sd and not p.requires_grad:
             del sd[name]
+    if step is not None and step.flat.P32 is not None:
+        for name, t in step.flat.master_state_dict().items():
+            key = name if name in sd else "module." + name
+            if key not in sd:
+                raise KeyError(f"get_checkpoint: master weight {name} is not a trainable entry of the model")
+            sd[key] = t
     return sd
+
+
+# --bf16_module names of the reference (train.py:126-163) whose modules are TRAINED: with fp32 master weights they would
+# need a partial master buffer, which this package does not implement.  vision_encoder / text_encoder are frozen and run in
+# bf16 here whatever --bf16_module says.
+TRAINABLE_BF16_MODULES = ("image_primary_projector", "image_wrist_projector", "perceiver_resampler", "causal_transformer",
+                          "image_decoder", "depth_decoder", "action_decoder", "dino_decoder", "sam_decoder")
+FROZEN_BF16_MODULES = ("vision_encoder", "text_encoder")
+
+
+def resolve_precision(args) -> str:
+    """"bf16" (parameters stored in bf16) or "fp32" (fp32 master weights, bf16 working copy) for `--precision`; anything
+    this package cannot honour raises SystemExit."""
+    if args.precision in ("bf16", "amp_bf16", "amp_bfloat16"):
+        return "bf16"
+    if args.precision != "fp32":
+        raise SystemExit(f"--precision {args.precision} is not supported: use fp32 (fp32 master weights, bf16 compute) "
+                         "or bf16")
+    spec = getattr(args, "bf16_module", "") or ""
+    trained = [m for m in TRAINABLE_BF16_MODULES if m in spec]      # the reference matches by substring
+    if trained:
+        raise SystemExit(f"--precision fp32 with --bf16_module naming trained modules ({', '.join(trained)}) is not "
+                         "supported: every trained parameter gets an fp32 master copy.  --bf16_module may name only "
+                         f"{' / '.join(FROZEN_BF16_MODULES)}")
+    unknown = [t for t in re.split(r"[\s,;]+", spec.strip()) if t and t not in FROZEN_BF16_MODULES]
+    if unknown:
+        raise SystemExit(f"--bf16_module: unknown module name(s) {unknown}; with --precision fp32 it may name only "
+                         f"{' / '.join(FROZEN_BF16_MODULES)}")
+    return "fp32"
 
 
 def main(args, loader=None):
     args.local_rank, args.rank, args.world_size = world_info_from_env()
+    precision = resolve_precision(args)
     device_id = init_distributed_device(args)
     random_seed(args.seed)                   # train.py:50: every rank builds the SAME initial model
-    if args.precision not in ("bf16", "amp_bf16", "amp_bfloat16"):
-        raise SystemExit("dreamvla_b200 kernels are bf16-only: run with --precision bf16")
     model = DreamVLA(finetune_type=args.finetune_type, clip_device="cpu", vit_checkpoint_path=args.vit_checkpoint_path,
                      **model_kwargs(args))
-    model = model.bfloat16()
     model.clip_model.requires_grad_(False)
     model.vision_encoder.requires_grad_(False)          # runs under no_grad in forward (dreamvla_model.py:670)
-    model = model.to(device_id)
-    model._init_model_type()
     ddp_model = _ModuleWrapper(model)
     random_seed(args.seed, args.rank)        # train.py:110: data order / dropout / diffusion draws differ per rank
     if loader is None:
@@ -187,10 +225,18 @@ def main(args, loader=None):
         opt_state = ck.get("optimizer_state_dict")
         sched.load_state_dict(ck["lr_scheduler_state_dict"])
         resume_from_epoch = ck["epoch"] + 1
+    # Checkpoints are loaded into the fp32 model, so with --precision fp32 values that bf16 cannot represent survive into
+    # the master weights; the model itself (the kernels' working copy) is bf16 in both modes.
+    master = None
+    if precision == "fp32":
+        master = {name: p.detach().clone() for name, p in model.named_parameters() if p.requires_grad}
+    model = model.bfloat16().to(device_id)
+    model._init_model_type()
     # The flat parameter / gradient / AdamW-moment buffers (the optimiser of this package) are built AFTER every checkpoint
     # load: parameters become views of one buffer, rank 0's copy is broadcast (DDP constructor semantics, train.py:173), and
     # a resumed run gets its moments and step count back (train.py:256).
-    state = TrainStep(model, StepConfig.from_args(args), world_size=args.world_size)
+    state = TrainStep(model, StepConfig.from_args(args), world_size=args.world_size, master=master)
+    del master
     model._dvla_train_step = state
     if opt_state is not None:
         if opt_state.get("format") != "dvla_flat_adamw_v1":
@@ -205,7 +251,7 @@ def main(args, loader=None):
         state = train_one_epoch_calvin(args=args, model=ddp_model, epoch=epoch, optimizer=None, lr_scheduler=sched,
                                        calvin_loader=loader, device_id=device_id, wandb=None)
         if args.rank == 0 and args.save_checkpoint and epoch % args.save_checkpoint_seq == 0 and epoch > args.start_save_checkpoint:
-            torch.save({"epoch": epoch, "model_state_dict": get_checkpoint(ddp_model),
+            torch.save({"epoch": epoch, "model_state_dict": get_checkpoint(ddp_model, state),
                         "optimizer_state_dict": state.flat.optimizer_state_dict(),
                         "lr_scheduler_state_dict": sched.state_dict()}, os.path.join(ckpt_dir, f"{epoch}.pth"))
     if args.rank == 0 and state is not None:
