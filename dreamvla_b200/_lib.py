@@ -78,6 +78,11 @@ class AdamWMasterArgs(C.Structure):
                 ("max_norm", _f32), ("grad_scale", _f32), ("zero_grad", _i32)]
 
 
+class ImageFnArgs(C.Structure):
+    _fields_ = [("frames", _vp), ("out", _vp), ("n", _i64), ("h", _i64), ("w", _i64), ("c", _i64), ("xbounds", _vp),
+                ("xcoeffs", _vp), ("ybounds", _vp), ("ycoeffs", _vp), ("lut", _vp), ("flip_vertical", _i32), ("out_dtype", _i32)]
+
+
 class DitBlockWeights(C.Structure):
     _fields_ = [(n, _vp) for n in ("qkv_w", "qkv_b", "proj_w", "proj_b", "fc1_w", "fc1_b", "fc2_w", "fc2_b")]
 
@@ -95,7 +100,7 @@ class DitSamplerArgs(C.Structure):
 EXPORTS = [
     "dvla_version", "dvla_last_error", "dvla_launch_count", "dvla_gemm", "dvla_gemm_plan", "dvla_gemm_plan_unit", "dvla_layernorm_fwd", "dvla_layernorm_bwd",
     "dvla_attn_fwd", "dvla_attn_bwd", "dvla_attn_mask_tiles", "dvla_colsum_accum", "dvla_accum_fp32_into_bf16",
-    "dvla_dropout", "dvla_act_bwd", "dvla_act_bwd_colsum", "dvla_cat_broadcast", "dvla_shift_crop", "dvla_resize_nearest", "dvla_mse_loss", "dvla_cosine_loss", "dvla_silog_stats", "dvla_silog_finish",
+    "dvla_dropout", "dvla_act_bwd", "dvla_act_bwd_colsum", "dvla_cat_broadcast", "dvla_shift_crop", "dvla_resize_nearest", "dvla_image_fn", "dvla_bicubic_taps", "dvla_bicubic_coeffs", "dvla_mse_loss", "dvla_cosine_loss", "dvla_silog_stats", "dvla_silog_finish",
     "dvla_sumsq", "dvla_adamw", "dvla_adamw_master", "dvla_grad_clip_scale", "dvla_attn_bwd_workspace_bytes", "dvla_silog_workspace_bytes",
     "dvla_gemm_workspace_bytes", "dvla_set_sm_budget", "dvla_dit_ddim_sample", "dvla_dit_sampler_workspace_bytes",
 ]
@@ -350,6 +355,65 @@ def resize_nearest(x, hout, wout, out_dtype=torch.float32):
     out = torch.empty((*x.shape[:-2], hout, wout), device=x.device, dtype=out_dtype)
     _check(load().dvla_resize_nearest(C.c_void_p(x.data_ptr()), C.c_void_p(out.data_ptr()), _i64(n), _i64(hin), _i64(win),
                                       _i64(hout), _i64(wout), C.c_int32(_DT[out_dtype]), _stream()), "dvla_resize_nearest")
+    return out
+
+
+IMAGE_FN_SIZE = 224
+
+
+def image_fn_geometry(h, w, size=IMAGE_FN_SIZE):
+    """torchvision `Resize(size)` (short side -> size, long side int(size * long / short)) + `CenterCrop(size)` of an h x w
+    frame -> (resized h, resized w, crop top, crop left); include/dvla.h dvla_image_fn."""
+    short, long = (w, h) if w <= h else (h, w)
+    new_long = int(size * long / short)
+    rh, rw = (new_long, size) if w <= h else (size, new_long)
+    return rh, rw, int(round((rh - size) / 2.0)), int(round((rw - size) / 2.0))
+
+
+def bicubic_coeffs(in_size, out_size, first, count):
+    """Pillow's bicubic bounds / int32 coefficients of outputs [first, first + count) of a line resized from in_size to
+    out_size (host only, no GPU): (bounds int32 [count, 2] = (first input pixel, taps used), coeffs int32 [count, taps])."""
+    lib = load()
+    taps = int(lib.dvla_bicubic_taps(_i64(in_size), _i64(out_size)))
+    _check(min(taps, 0), "dvla_bicubic_taps")
+    bounds = torch.zeros((count, 2), dtype=torch.int32)
+    coeffs = torch.zeros((count, taps), dtype=torch.int32)
+    _check(lib.dvla_bicubic_coeffs(_i64(in_size), _i64(out_size), _i64(first), _i64(count), C.c_void_p(bounds.data_ptr()),
+                                   C.c_void_p(coeffs.data_ptr())), "dvla_bicubic_coeffs")
+    return bounds, coeffs
+
+
+_image_fn_tables = {}
+
+
+def image_fn_tables(h, w, device):
+    """Device copies of the coefficient tables of an h x w frame ((xbounds, xcoeffs, ybounds, ycoeffs)), built once per
+    (device, h, w).  The first call for a frame size uploads them: make it outside CUDA-graph capture."""
+    key = (device.index if device.index is not None else torch.cuda.current_device(), int(h), int(w))
+    t = _image_fn_tables.get(key)
+    if t is None:
+        rh, rw, top, left = image_fn_geometry(h, w)
+        xb, xc = bicubic_coeffs(w, rw, left, IMAGE_FN_SIZE)
+        yb, yc = bicubic_coeffs(h, rh, top, IMAGE_FN_SIZE)
+        t = _image_fn_tables[key] = tuple(v.to(device) for v in (xb, xc, yb, yc))
+    return t
+
+
+def image_fn(frames, lut, out_dtype=torch.float32, flip_vertical=False):
+    """CLIP `_transform(224)` of uint8 frames [n, h, w, 3] (contiguous, HWC) -> [n, 3, 224, 224] `out_dtype` (fp32 / bf16):
+    Pillow-exact bicubic resize of the short side to 224, centre crop, then out = lut[c, value] with lut fp32 [3, 256]
+    (include/dvla.h dvla_image_fn).  flip_vertical reads every frame bottom-up."""
+    _need_cuda(frames, lut)
+    assert frames.dtype == torch.uint8 and frames.dim() == 4 and frames.is_contiguous(), (frames.dtype, frames.shape)
+    assert lut.dtype == torch.float32 and lut.shape == (3, 256) and lut.is_contiguous()
+    n, h, w, c = frames.shape
+    out = torch.empty((n, 3, IMAGE_FN_SIZE, IMAGE_FN_SIZE), device=frames.device, dtype=out_dtype)
+    if n == 0:
+        return out
+    xb, xc, yb, yc = image_fn_tables(h, w, frames.device)
+    a = ImageFnArgs(frames.data_ptr(), out.data_ptr(), n, h, w, c, xb.data_ptr(), xc.data_ptr(), yb.data_ptr(), yc.data_ptr(),
+                    lut.data_ptr(), int(bool(flip_vertical)), _DT[out_dtype])
+    _check(load().dvla_image_fn(C.byref(a), _stream()), "dvla_image_fn")
     return out
 
 

@@ -18,6 +18,8 @@ SOURCES = ["gemm_sm90.cu", "attention.cu", "attention_small.cu", "norm_act.cu", 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
+    # host code keeps separate multiplies and adds (no FMA contraction): dvla_bicubic_coeffs must round like Pillow's C
+    "-Xcompiler", "-ffp-contract=off",
 ]
 
 

@@ -40,6 +40,9 @@ int shift_crop_dispatch(const void* x, void* out, const int32_t* shifts, int64_t
                         int32_t in_dtype, int32_t out_dtype, cudaStream_t s);
 int resize_nearest_dispatch(const float* x, void* out, int64_t n, int64_t hin, int64_t win, int64_t hout, int64_t wout,
                             int32_t out_dtype, cudaStream_t s);
+int image_fn_dispatch(const dvla_image_fn_args* a, cudaStream_t s);
+int bicubic_taps(int64_t in_size, int64_t out_size);
+int bicubic_coeffs(int64_t in_size, int64_t out_size, int64_t first, int64_t count, int32_t* bounds, int32_t* coeffs);
 int gemm_plan(const dvla_gemm_args* a, dvla_gemm_plan_info* out);
 int gemm_plan_unit(const dvla_gemm_plan_info* plan, int unit, int* tile, int* kb0, int* kb1, int* slot, int* split);
 int layernorm_fwd_dispatch(const dvla_layernorm_fwd_args* a, cudaStream_t stream);
@@ -117,6 +120,11 @@ int dvla_shift_crop(const void* x, void* out, const int32_t* shifts_xy, int64_t 
 int dvla_resize_nearest(const float* x, void* out, int64_t n, int64_t hin, int64_t win, int64_t hout, int64_t wout,
                         int32_t out_dtype, void* stream) {
   return resize_nearest_dispatch(x, out, n, hin, win, hout, wout, out_dtype, S(stream));
+}
+int dvla_image_fn(const dvla_image_fn_args* a, void* stream) { return image_fn_dispatch(a, S(stream)); }
+int32_t dvla_bicubic_taps(int64_t in_size, int64_t out_size) { return bicubic_taps(in_size, out_size); }
+int dvla_bicubic_coeffs(int64_t in_size, int64_t out_size, int64_t first, int64_t count, int32_t* bounds, int32_t* coeffs) {
+  return bicubic_coeffs(in_size, out_size, first, count, bounds, coeffs);
 }
 int dvla_act_bwd_colsum(const void* dy, const void* pre, void* dx, int64_t rows, int64_t N, int32_t act, float* colsum,
                         void* stream) {

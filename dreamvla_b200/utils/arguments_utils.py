@@ -55,7 +55,8 @@ _FLAGS = [
 # added by this repo (not in the reference)
 # --device_augment: apply the collator's RandomShiftsAug (--rgb_pad / --gripper_pad / --traj_cons, reference
 # utils/data_utils.py:1337-1354) on the GPU to the transferred batch (utils/data_utils.py here); the loader must then be built
-# WITHOUT pads so that the augmentation is not applied twice.
+# WITHOUT pads so that the augmentation is not applied twice.  A loader may ship raw uint8 camera frames instead of
+# preprocessed ones (no flag: the dtype decides); CLIP's image transform then runs on the device before the shifts.
 # --exchange_on_boundary_only: with gradient accumulation, all-reduce + clip once per optimiser step instead of the
 # reference's every-micro-step exchange and in-place clip (utils/train_utils.py:599-600); a different update, opt-in.
 _EXTRA = [("--synthetic_steps", int, 0), ("--cuda_graph", "flag", False), ("--synthetic_rollout_steps", int, 0),

@@ -1,5 +1,6 @@
 """Action-inference wrapper -- mirror of reference utils/eval_utils_calvin.py:48-147 (`ModelWrapper.step`), without the
-simulator (out of scope).  Inputs are already-preprocessed tensors (CLIP image preprocessing / tokenisation are data-side).
+simulator (out of scope).  Images are raw uint8 camera frames (CLIP's image transform then runs on the device) or
+already-preprocessed tensors; tokenisation is data-side.
 
 Semantics kept (reference :107-145): growing-then-sliding window of `history_len` frames, window padded by repeating the
 last frame, the instruction tokens of the FIRST step frozen for the episode and repeated over the window, gripper
@@ -19,7 +20,10 @@ from __future__ import annotations
 
 from collections import deque
 
+import numpy as np
 import torch
+
+from .data_utils import preprocess_image
 
 
 class RolloutEngine:
@@ -152,14 +156,27 @@ class RolloutEngine:
         return out
 
     # ---- one env step -----------------------------------------------------------------------------------------------------
+    def _frame(self, image, flip_vertical=False):
+        """-> [1, 1, 3, 224, 224] in the cast dtype on the device.  A raw uint8 [h, w, 3] frame (numpy array or tensor, as the
+        simulator returns it) is uploaded as bytes and put through CLIP's image transform on the device (`preprocess_image`,
+        the reference's `image_process_fn`, :82-90); a preprocessed [3, 224, 224] tensor is only moved and cast."""
+        if isinstance(image, np.ndarray):
+            image = torch.from_numpy(np.ascontiguousarray(image))
+        if image.dtype != torch.uint8:
+            return image.to(self.device, self.cast_type).view(1, 1, 3, 224, 224)
+        out_dtype = self.cast_type if self.cast_type in (torch.float32, torch.bfloat16) else torch.float32
+        x = preprocess_image(image.to(self.device), out_dtype, flip_vertical)
+        return x.to(self.cast_type).view(1, 1, 3, 224, 224)
+
     @torch.no_grad()
-    def infer(self, image_static, image_gripper, state_vec, text_tokens, sample_noise=None):
+    def infer(self, image_static, image_gripper, state_vec, text_tokens, sample_noise=None, flip_static=False):
         """Push one observation, return (arm [steps, 6], gripper [steps, 1], num_step) of the SELECTED timestep.
-        sample_noise: the DDIM start noise -- [S, steps, 7] (the full-window draw of the reference, :944) or [1, steps, 7]
-        (the selected row only)."""
+        image_*: preprocessed [3, 224, 224] tensors or raw uint8 [h, w, 3] frames (see `_frame`; `flip_static` flips a raw
+        static frame upside down first).  sample_noise: the DDIM start noise -- [S, steps, 7] (the full-window draw of the
+        reference, :944) or [1, steps, 7] (the selected row only)."""
         dev = self.device
-        img = image_static.to(dev, self.cast_type).view(1, 1, 3, 224, 224)
-        grip = image_gripper.to(dev, self.cast_type).view(1, 1, 3, 224, 224)
+        img = self._frame(image_static, flip_static)
+        grip = self._frame(image_gripper)
         st = state_vec.to(dev, self.cast_type).view(1, 1, -1)
         assert st.shape[-1] == self.state_dim, f"state has {st.shape[-1]} dims, the model expects {self.state_dim}"
         if self.text_token is None:                              # frozen for the episode (:110-113)
@@ -194,7 +211,8 @@ class ModelWrapper(RolloutEngine):
 
     @torch.no_grad()
     def step(self, image_static, image_gripper, robot_obs, text_tokens, sample_noise=None):
-        """image_* [3,224,224] preprocessed, robot_obs [15], text_tokens int [77] -> action [7] (fp16 numpy like the reference)."""
+        """image_* raw uint8 [h, w, 3] frames (`obs["rgb_obs"]["rgb_static" / "rgb_gripper"]`) or [3,224,224] preprocessed,
+        robot_obs [15], text_tokens int [77] -> action [7] (fp16 numpy like the reference)."""
         st = robot_obs.reshape(-1)
         st = torch.cat([st[:6], st[-1:]], dim=-1)                          # :104
         arm, gripper, _ = self.infer(image_static, image_gripper, st, text_tokens, sample_noise)

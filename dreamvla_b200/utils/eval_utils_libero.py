@@ -1,5 +1,5 @@
 """LIBERO action-inference wrapper -- mirror of reference utils/eval_utils_libero.py:43-179 (`ModelWrapper.step`), without the
-MuJoCo simulator (out of scope).  Inputs are already-preprocessed tensors.
+MuJoCo simulator (out of scope).  Images are raw uint8 camera frames or already-preprocessed tensors (see `ModelWrapper.step`).
 
 What differs from the CALVIN wrapper (utils/eval_utils_calvin.py here), all kept from the reference:
   * state = [eef_pos(3), euler_xyz(eef_quat)(3), g] with g = the gripper command of the PREVIOUS action (initially -1), or
@@ -66,10 +66,11 @@ class ModelWrapper(RolloutEngine):
 
     @torch.no_grad()
     def step(self, image_agentview, image_eye_in_hand, eef_pos, eef_quat, gripper_qpos, text_tokens, timestep, sample_noise=None):
-        """One env step -> action [7] numpy; see module docstring.  image_* are [3,224,224] preprocessed tensors (the
-        reference flips the agent view vertically before preprocessing, :96 -- data-side)."""
+        """One env step -> action [7] numpy; see module docstring.  image_* are the raw uint8 [h, w, 3] camera frames
+        (`obs["agentview_image"]`, `obs["robot0_eye_in_hand_image"]`) or [3,224,224] preprocessed tensors.  A raw agent view
+        is flipped vertically before preprocessing, as the reference does (:96); a preprocessed one is taken as it is."""
         state = torch.from_numpy(self.build_state(eef_pos, eef_quat, gripper_qpos))
-        arm, gripper, _ = self.infer(image_agentview, image_eye_in_hand, state, text_tokens, sample_noise)
+        arm, gripper, _ = self.infer(image_agentview, image_eye_in_hand, state, text_tokens, sample_noise, flip_static=True)
         if self.use_ensembling:
             action = torch.cat((arm, gripper), dim=-1).unsqueeze(0)           # (1, action_pred_steps, 7)   :165
             self.all_time_actions[timestep:timestep + 1, timestep:timestep + self.action_pred_steps] = action.to(self.all_time_actions.dtype)

@@ -720,7 +720,9 @@ class _DeviceSlot:
 def prefetch_to_device(loader, device, to_host_dict=None, dtype=torch.bfloat16, slots=2):
     """Iterate `loader`, yielding each batch as a dict of DEVICE tensors; the host->device copies of batch i+1 are enqueued on a
     copy stream right after the consumer has enqueued step i, so a step's input transfer (193 MB at C2, ~3.5 ms over PCIe 5
-    x16) runs beside that step's kernels.  The host stays at most one step ahead of the device (see `stage`).
+    x16) runs beside that step's kernels.  The host stays at most one step ahead of the device (see `stage`).  A loader that
+    ships raw uint8 frames moves their bytes unchanged (49 KB per 128x128 frame instead of 602 KB of fp32 224x224);
+    `data_utils.prepare_batch` preprocesses them on the device.
 
     `to_host_dict(item)` maps a loader item to a dict of host tensors (default: the item itself); pinned host memory is
     needed for the copy to be asynchronous.  The device buffers are `slots` persistent sets reused round-robin (no allocator
@@ -791,13 +793,13 @@ def train_one_epoch_calvin(args, model, epoch, calvin_loader, optimizer, lr_sche
     accum = args.gradient_accumulation_steps
     state.micro = 0           # the reference counts accumulation windows from the start of each epoch (:602)
     graphed = getattr(core, "_dvla_graphed_step", None)
-    device_augment = bool(getattr(args, "device_augment", False)) and (getattr(args, "rgb_pad", -1) != -1
-                                                                        or getattr(args, "gripper_pad", -1) != -1)
+    from .data_utils import prepare_batch
     for num_steps, batch in enumerate(prefetch_to_device(calvin_loader, dev, batch_to_host_dict)):
         data_time_m.update(time.time() - end)
-        if device_augment:        # the collator's random shifts (reference data_utils.py:1337-1354), on the device
-            from .data_utils import augment_batch
-            batch = augment_batch(batch, args.rgb_pad, args.gripper_pad, bool(getattr(args, "traj_cons", False)))
+        # raw uint8 frames -> CLIP image_fn, then (--device_augment) the collator's random shifts (reference
+        # data_utils.py:1311-1312, :1337-1354), on the device and before the CUDA-graph step's static-buffer copy
+        batch = prepare_batch(batch, getattr(args, "rgb_pad", -1), getattr(args, "gripper_pad", -1),
+                              bool(getattr(args, "traj_cons", False)), bool(getattr(args, "device_augment", False)))
         lr = lr_scheduler.get_last_lr()[0] if lr_scheduler is not None else args.learning_rate
         if use_graph and graphed is None and state.total_micro > 0:
             graphed = GraphedTrainStep(state, batch, warmup=0)

@@ -304,6 +304,42 @@ int dvla_shift_crop(const void* x, void* out, const int32_t* shifts_xy, int64_t 
 int dvla_resize_nearest(const float* x_f32, void* out, int64_t n, int64_t hin, int64_t win, int64_t hout, int64_t wout,
                         int32_t out_dtype, void* stream);
 
+/* dvla_image_fn = CLIP's image transform `image_processor` (openai CLIP _transform(224): Resize(224, BICUBIC), CenterCrop(224),
+ * ToTensor, Normalize) of 8-bit RGB frames, as the collator (utils/data_utils.py:175-179, :1311-1312) and the rollout wrappers
+ * (utils/eval_utils_calvin.py:82-90, utils/eval_utils_libero.py:94-106) apply it through Pillow + torchvision, bit for bit:
+ *   - resize: the short side becomes 224, the long side int(224 * long / short); a frame whose short side is 224 is not
+ *     resampled.  Crop offsets int(round((size - 224) / 2)), Python's round (half to even).  Only the crop is computed.
+ *   - Pillow's 8-bit resampling: horizontal pass, then vertical, each value clip8(2^21 + sum pixel * coeff) rounded to uint8
+ *     between the passes; clip8(v) = 0 for v <= 0, 255 for v >= 2^30, v >> 22 otherwise.  Coefficient tables as
+ *     dvla_bicubic_coeffs fills them: x* = (w, resized w, crop left, 224), y* = (h, resized h, crop top, 224).
+ *   - out[i, ch, y, x] = lut[ch * 256 + v] for the resampled value v; the caller computes lut = (arange(256) / 255 - mean) / std
+ *     (fp32 [3, 256]), so the output is ToTensor + Normalize's own arithmetic.
+ * frames: uint8 [n, h, w, c] contiguous (HWC, what datasets and simulators hold), c must be 3, 1 <= h, w <= 3584 (a downscale
+ * of at most 16x); out: [n, 3, 224, 224] fp32 / bf16 (out_dtype 0 / 1), 16-byte aligned.  flip_vertical != 0 reads the frame
+ * bottom-up (LIBERO's agent view, utils/eval_utils_libero.py:96).  n = 0 is a no-op.  Bad arguments return DVLA_ERR_INVALID
+ * without launching. */
+typedef struct {
+  const uint8_t* frames;
+  void* out;
+  int64_t n, h, w, c;
+  const int32_t* xbounds; const int32_t* xcoeffs;     /* [224, 2], [224, dvla_bicubic_taps(w, resized w)] */
+  const int32_t* ybounds; const int32_t* ycoeffs;     /* [224, 2], [224, dvla_bicubic_taps(h, resized h)] */
+  const float* lut;                                   /* [3, 256] */
+  int32_t flip_vertical;
+  int32_t out_dtype;
+} dvla_image_fn_args;
+int dvla_image_fn(const dvla_image_fn_args* args, void* stream);
+
+/* Pillow's bicubic resampling coefficients (Resample.c precompute_coeffs + normalize_coeffs_8bpc, a = -0.5, support
+ * 2 * max(in/out, 1), double arithmetic, normalised by their sum, rounded half away from zero at 2^22) of a line of in_size
+ * pixels resized to out_size, for the outputs [first, first + count).  Host code only, no CUDA call.
+ *   bounds[2i] = first input pixel of output first + i, bounds[2i + 1] = its number of taps;
+ *   coeffs[i * taps + k] = int32 coefficient of tap k, 0 past the used taps;  taps = dvla_bicubic_taps(in_size, out_size).
+ * in_size == out_size is the identity (one tap of 2^22): Pillow skips a pass whose size does not change.
+ * dvla_bicubic_taps returns the number of coefficients per output (Pillow's ksize), or a negative dvla_status. */
+int32_t dvla_bicubic_taps(int64_t in_size, int64_t out_size);
+int dvla_bicubic_coeffs(int64_t in_size, int64_t out_size, int64_t first, int64_t count, int32_t* bounds, int32_t* coeffs);
+
 /* SM budget of the persistent GEMM kernels (one CTA / CTA pair per SM).  0 = all SMs (default).  The data-parallel train
  * step lowers it by the number of CTAs the NCCL all-reduce occupies while gradient exchange overlaps the backward pass
  * (train.py:173 DDP overlap), so that every GEMM CTA is resident at once.  Returns the previous value.  Process-wide. */
