@@ -546,13 +546,4 @@ def dit_ddim_sample(net, diffusion, z, noise, cfg_scale):
     a.n_steps, a.cfg_scale = n_steps, float(cfg_scale)
     a.workspace, a.workspace_bytes = ws.data_ptr(), ws_bytes
     _check(load().dvla_dit_ddim_sample(C.byref(a), _stream()), "dvla_dit_ddim_sample")
-    if os.environ.get("DVLA_DIT_TRACE") == "1":       # diagnostic: phase boundaries of CTA 0 (ns, globaltimer)
-        torch.cuda.synchronize()
-        M = 2 * bs * 2 * T
-        used = 4 * (2 * M * H + M * 3 * H + M * mlp + 2 * n_steps * H + (bs * T + 1) * H)
-        off = ((ws.data_ptr() + used + 15) & ~15) - ws.data_ptr()
-        tr = ws[off:off + 256 * 8].view(torch.int64).cpu().tolist()
-        n = tr[0]
-        st = tr[1:1 + n]
-        print("[dit trace] stamps:", n, "deltas us:", [round((b - a) / 1e3, 1) for a, b in zip(st[:-1], st[1:])], flush=True)
     return out

@@ -11,7 +11,6 @@
 //   attn_bwd_dkv_kernel grid (ceil(Lk/64), H, B): per key tile, loops over query tiles, S^T/dP^T formulation
 //   attn_bwd_dq_kernel  grid (ceil(Lq/64), H, B): per query tile, loops over key tiles
 // Masking: tile_flags[qt, kt] in {0 skip, 1 partial, 2 full}; partial tiles test bits of mask[i, j/32].
-#include <stdlib.h>
 #include <string.h>
 
 #include <mutex>
@@ -1012,10 +1011,6 @@ static bool strides_ok(const void* ptr, long long sb, long long ss, long long sh
 bool attn_small_applicable(int64_t Lq, int64_t Lk, const void* mask, float dropout_p);   // attention_small.cu
 int attn_small_fwd_dispatch(const dvla_attn_fwd_args* a, cudaStream_t s);
 int attn_small_bwd_dispatch(const dvla_attn_bwd_args* a, cudaStream_t s);
-static bool attn_small_enabled() {
-  static const bool on = [] { const char* e = getenv("DVLA_ATTN_SMALL"); return !(e && e[0] == '0'); }();   // thread-safe init
-  return on;
-}
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
@@ -1084,7 +1079,7 @@ int attn_fwd_dispatch(const dvla_attn_fwd_args* a, cudaStream_t s) {
     }
     return attn_small_fwd_dispatch(a, s);
   }
-  if (attn_small_enabled() && attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p))
+  if (attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p))
     return attn_small_fwd_dispatch(a, s);
   AttnParams p;
   memset(&p, 0, sizeof(p));
@@ -1162,7 +1157,7 @@ int attn_bwd_dispatch(const dvla_attn_bwd_args* a, cudaStream_t s) {
     }
     return attn_small_bwd_dispatch(a, s);
   }
-  if (attn_small_enabled() && attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p))
+  if (attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p))
     return attn_small_bwd_dispatch(a, s);          // writes delta itself
   const long long rows = (long long)p.B * p.H * p.Lq;
   attn_delta_kernel<<<(unsigned)((rows * 8 + 255) / 256), 256, 0, s>>>(p);

@@ -17,7 +17,6 @@
 // residual stream in bf16), so results agree with it to bf16 rounding, not bit for bit (tests/test_rollout_gpu.py).
 #include <cooperative_groups.h>
 
-#include <stdlib.h>
 #include <string.h>
 
 #include "common.cuh"
@@ -52,7 +51,6 @@ struct DitSamplerParams {
   float cfg_scale;
   int bs, T, C, H, heads, token, mlp, freq;
   float *h0, *h1, *qkv, *u, *te, *t1, *ze;     // fp32 scratch (global, L2 resident)
-  unsigned long long* trace;                   // optional: globaltimer stamps of CTA 0 at phase boundaries (DVLA_DIT_TRACE)
 };
 
 __device__ __forceinline__ float warp_sum_f(float v) {
@@ -265,16 +263,6 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dit_ddim_sample_kernel(const __
   float* eps_s = xcur + bs * T * C;                                           // [nseq][T][C] final-layer outputs
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int gtid = blockIdx.x * DS_THREADS + tid, gthreads = gridDim.x * DS_THREADS;
-  int tr_n = 0;
-  auto stamp = [&]() {
-    if (p.trace && blockIdx.x == 0 && tid == 0 && tr_n < 255) {
-      unsigned long long t;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-      p.trace[1 + tr_n++] = t;
-      p.trace[0] = tr_n;
-    }
-  };
-  stamp();
 
   // ---- prologue A: timestep-frequency features -> t1 = silu(W0 f + b0) for all steps;  ze = Wz z + bz for the bs*T condition
   //      rows and for the `uncondition` vector (row bs*T)
@@ -303,7 +291,6 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dit_ddim_sample_kernel(const __
   __syncthreads();
   skinny_gemm<MROWS>(Xs, p.n_steps, H, p.t2_w, p.t2_b, H, p.te, H, EPI_STORE);
   grid.sync();
-  stamp();
 
   for (int step = p.n_steps - 1, it = 0; step >= 0; --step, ++it) {
     float* h = (it & 1) ? p.h1 : p.h0;
@@ -325,16 +312,13 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dit_ddim_sample_kernel(const __
       h[i] = v + __bfloat162float(p.pos[tok * H + c]);
     }
     grid.sync();
-    stamp();
     for (int l = 0; l < p.depth; ++l) {
       const DitBlockW& w = p.blk[l];
       // ---- P1: qkv = LN(h) Wqkv^T + b
       stage_layernorm(Xs, h, M, H);
       __syncthreads();
       skinny_gemm<MROWS>(Xs, M, H, w.qkv_w, w.qkv_b, 3 * H, p.qkv, 3 * H, EPI_STORE);
-      if (it == 0 && l < 2) stamp();
       grid.sync();
-      if (it == 0 && l < 2) stamp();
       // ---- P2: attention (every CTA computes all (sequence, head) pairs: 6x6 scores each) -> O in shared; h += O Wproj^T + b
       {
         bf16* Os = Xs;                                                     // [M][H] bf16
@@ -372,30 +356,20 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dit_ddim_sample_kernel(const __
           }
         }
         __syncthreads();
-        if (it == 0 && l < 2) stamp();
         skinny_gemm<MROWS>(Os, M, H, w.proj_w, w.proj_b, H, h, H, EPI_ACC);
       }
-      if (it == 0 && l < 2) stamp();
       grid.sync();
-      if (it == 0 && l < 2) stamp();
       // ---- P3: u = gelu_tanh(LN(h) Wfc1^T + b)
       stage_layernorm(Xs, h, M, H);
       __syncthreads();
-      if (it == 0 && l < 2) stamp();
       skinny_gemm<MROWS>(Xs, M, H, w.fc1_w, w.fc1_b, p.mlp, p.u, p.mlp, EPI_GELU);
-      if (it == 0 && l < 2) stamp();
       grid.sync();
-      if (it == 0 && l < 2) stamp();
       // ---- P4: h += u Wfc2^T + b
       stage_rows(Xs, p.u, M * p.mlp);
       __syncthreads();
-      if (it == 0 && l < 2) stamp();
       skinny_gemm<MROWS>(Xs, M, p.mlp, w.fc2_w, w.fc2_b, H, h, H, EPI_ACC);
-      if (it == 0 && l < 2) stamp();
       grid.sync();
-      if (it == 0 && l < 2) stamp();
     }
-    if (it < 3) stamp();
     // ---- final layer on the action rows + guidance + DDIM update: redundantly in every CTA (x stays in shared memory).
     //      h of this step is not written again before two more grid barriers (the next step uses the other h buffer).
     {
@@ -470,8 +444,6 @@ int dit_ddim_sample_dispatch(const dvla_dit_sampler_args* a, cudaStream_t s) {
   p.te = ws; ws += p.n_steps * H;
   p.t1 = ws; ws += p.n_steps * H;
   p.ze = ws; ws += (bs * T + 1) * H;
-  static const bool want_trace = [] { const char* v = getenv("DVLA_DIT_TRACE"); return v && v[0] == '1'; }();
-  p.trace = want_trace ? reinterpret_cast<unsigned long long*>((reinterpret_cast<uintptr_t>(ws) + 15) & ~static_cast<uintptr_t>(15)) : nullptr;   // 256 x u64 behind the scratch buffers
   int widest = p.mlp > p.token ? p.mlp : p.token;
   if (p.freq > widest) widest = p.freq;
   int rows = M > bs * T + 1 ? M : bs * T + 1;
@@ -493,11 +465,8 @@ int dit_ddim_sample_dispatch(const dvla_dit_sampler_args* a, cudaStream_t s) {
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
   if (!coop) { set_error("dit_ddim_sample: device has no cooperative launch"); return DVLA_ERR_UNSUPPORTED; }
-  static const int env_ctas = [] { const char* v = getenv("DVLA_DIT_CTAS"); return v ? atoi(v) : 0; }();
-  int ctas = num_sms();
-  if (env_ctas > 0 && env_ctas < ctas) ctas = env_ctas;
   void* args[] = {const_cast<DitSamplerParams*>(&p)};
-  cudaError_t e = cudaLaunchCooperativeKernel(kern, dim3(ctas), dim3(DS_THREADS), args, smem, s);
+  cudaError_t e = cudaLaunchCooperativeKernel(kern, dim3(num_sms()), dim3(DS_THREADS), args, smem, s);
   if (e != cudaSuccess) { set_error("dit_ddim_sample launch: %s", cudaGetErrorString(e)); return DVLA_ERR_CUDA; }
   count_launch();
   return DVLA_OK;
@@ -507,5 +476,5 @@ int dit_ddim_sample_dispatch(const dvla_dit_sampler_args* a, cudaStream_t s) {
 
 extern "C" int64_t dvla_dit_sampler_workspace_bytes(int64_t batch, int64_t T, int64_t hidden, int64_t mlp, int64_t n_steps) {
   const int64_t M = 2 * batch * 2 * T;
-  return 4 * (2 * M * hidden + M * 3 * hidden + M * mlp + 2 * n_steps * hidden + (batch * T + 1) * hidden) + 256 * 8 + 16;
+  return 4 * (2 * M * hidden + M * 3 * hidden + M * mlp + 2 * n_steps * hidden + (batch * T + 1) * hidden);
 }

@@ -750,23 +750,10 @@ static bool splitk_enabled() {
 
 static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
-// DVLA_GEMM_TAIL=0 disables the K-split tail (every unit of a plain GEMM is then a whole tile)
-static bool tail_enabled() {
-  static const bool on = [] { const char* e = getenv("DVLA_GEMM_TAIL"); return !(e && !strcmp(e, "0")); }();
-  return on;
-}
-// split-K weight gradients: partial sums added with red.global.add.bf16x2 (default), or with DVLA_GEMM_SPLITK=fp32 the same
-// fp32 slices + ordered fix-up as the tail: one bf16 rounding per accumulation and a reproducible summation order, at the
-// cost of the last unit's read-back of the other splits' slices
-static bool splitk_fp32() {
-  static const bool on = [] { const char* e = getenv("DVLA_GEMM_SPLITK"); return e && !strcmp(e, "fp32"); }();
-  return on;
-}
 // workspace = [16384 arrival counters (64 KB), zero between launches] [fp32 partial tiles: 128 x 128 x 4 bytes per CTA and split]
 constexpr int64_t TAIL_CNT_BYTES = 65536;
-constexpr int64_t TAIL_WS_SLICES = 1024;             // 128 x 128 fp32 slices (64 MB): a split tail wave needs <= 132 (one
-                                                     // per SM); fp32 split-K of a 4096 x 1024 weight gradient (256 tiles)
-                                                     // in four splits needs all 1024
+constexpr int64_t TAIL_WS_SLICES = 132;              // 128 x 128 fp32 slices (8.25 MB): a split tail wave needs <= 132 (one
+                                                     // per SM)
 int64_t gemm_workspace_bytes() { return TAIL_CNT_BYTES + TAIL_WS_SLICES * BM * BN * 4; }
 
 static bool tail_fits(const dvla_gemm_args* a, long long tail_tiles, int splits) {
@@ -774,15 +761,10 @@ static bool tail_fits(const dvla_gemm_args* a, long long tail_tiles, int splits)
   return tail_tiles * NUM_EPI_WARPS * 4 <= TAIL_CNT_BYTES &&
          TAIL_CNT_BYTES + tail_tiles * splits * (long long)BM * BN * 4 <= a->workspace_bytes;
 }
-static void set_tail(GemmParams& p, const dvla_gemm_args* a, int first, int splits, int kbps) {
-  p.tail_first = first; p.tail_splits = splits; p.tail_kbps = kbps;
-  p.tail_cnt = reinterpret_cast<unsigned*>(a->workspace);
-  p.tail_ws = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(a->workspace) + TAIL_CNT_BYTES);
-}
 // The tiles of a partly filled last wave are cut along K (see map_unit).  Model, in k-block times of one tile: a unit costs
 // its k-blocks + c0 (fill / drain / epilogue); a tail unit additionally the fp32 round trip through L2 (c_fix).
 static void plan_tail(GemmParams& p, const dvla_gemm_args* a, long long total_tiles, int slots) {
-  if (!tail_enabled() || !p.staged_ok || p.k_splits != 1 || total_tiles <= 0) return;
+  if (!p.staged_ok || p.k_splits != 1 || total_tiles <= 0) return;
   const long long full_waves = total_tiles / slots;
   const long long rem = total_tiles - full_waves * slots;
   // Only GEMMs of at least one full wave: a row's result then depends on M only for the large training GEMMs.  Below one
@@ -802,7 +784,9 @@ static void plan_tail(GemmParams& p, const dvla_gemm_args* a, long long total_ti
   const float with_tail = (float)full_waves * ((float)p.num_k_blocks + c0) + (float)kbps + c0 + c_fix;
   if (with_tail > 0.93f * now) return;
   if (!tail_fits(a, rem, tsp)) return;
-  set_tail(p, a, (int)(full_waves * slots), tsp, kbps);
+  p.tail_first = (int)(full_waves * slots); p.tail_splits = tsp; p.tail_kbps = kbps;
+  p.tail_cnt = reinterpret_cast<unsigned*>(a->workspace);
+  p.tail_ws = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(a->workspace) + TAIL_CNT_BYTES);
 }
 
 int gemm_dispatch(const dvla_gemm_args* a, cudaStream_t stream) {
@@ -879,17 +863,10 @@ int gemm_dispatch(const dvla_gemm_args* a, cudaStream_t stream) {
       if (t < best * 0.97f) { best = t; best_s = sp; }
     }
     if (best_s > 1) {
-      const int kbps = (p.num_k_blocks + best_s - 1) / best_s;
-      if (splitk_fp32() && tail_fits(a, tiles, best_s)) {
-        // every tile is split; the partial sums meet in fp32 slices and the last unit adds the complete product to the
-        // gradient (out = residual = G): ONE bf16 rounding per accumulation instead of one per split, fixed summation order
-        set_tail(p, a, 0, best_s, kbps);
-      } else {
-        p.k_splits = best_s;
-        p.kb_per_split = kbps;
-        p.atomic_out = 1;
-        p.residual = nullptr;
-      }
+      p.k_splits = best_s;
+      p.kb_per_split = (p.num_k_blocks + best_s - 1) / best_s;
+      p.atomic_out = 1;
+      p.residual = nullptr;
       return launch_tc_any(a, p, stream);
     }
   }

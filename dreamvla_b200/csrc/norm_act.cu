@@ -1,8 +1,5 @@
 // HBM-bound row kernels: LayerNorm fwd/bwd, column sums (bias grads), dropout, activation backward, fp32->bf16 folds.
 // One warp per row, 16-byte vector accesses, grids sized against the SM count.
-#include <stdlib.h>
-#include <string.h>
-
 #include "common.cuh"
 #include "../../include/dvla.h"
 
@@ -331,8 +328,7 @@ int layernorm_bwd_dispatch(const dvla_layernorm_bwd_args* a, cudaStream_t stream
   if (a->rows <= 0) return DVLA_OK;
   const int nv = (int)((a->D + 255) / 256);
   long long blocks = (a->rows + 7) / 8;
-  static const bool v2_on = [] { const char* e = getenv("DVLA_LN_BWD"); return !(e && !strcmp(e, "v1")); }();
-  if (v2_on && a->D % 256 == 0 && (a->dgamma || a->dbeta) && a->rows >= 2048) {
+  if (a->D % 256 == 0 && (a->dgamma || a->dbeta) && a->rows >= 2048) {
     const long long cap3 = 2LL * num_sms();
     if (blocks > cap3) blocks = cap3;
     const size_t smem = (size_t)8 * 2 * a->D * sizeof(float);

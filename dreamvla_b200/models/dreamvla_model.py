@@ -75,7 +75,7 @@ class _WorldDecoder(nn.Module):
 
     Reference computation per sequence: x = cat(projector(queries) [n_per], mask_token x n_mask) + pos_emb -> 2 timm Blocks
     -> LayerNorm -> Linear on the n_mask rows.  95 % of the rows are mask tokens, and `mask_token + pos_emb[n_per:]` does not
-    depend on the sequence (SURVEY §8 f-4), which is used twice (DVLA_DECODER_ALGEBRA=0 turns both off):
+    depend on the sequence (SURVEY §8 f-4), which is used twice:
       * shared first block input: LayerNorm-1 and the QKV projection of the mask rows of block 0 are computed ONCE per call
         ([n_mask, D] rows instead of n_seq * n_mask); the per-sequence rows are the n_per query rows only;
       * identical mask rows: if all mask rows of pos_emb are equal (the SAM head: zero position embedding, reference
@@ -84,7 +84,6 @@ class _WorldDecoder(nn.Module):
         row's key / value n_mask times; the prediction of that row is every mask row's prediction.
     Both are identities in exact arithmetic; in bf16 only summation orders change."""
 
-    ALGEBRA = os.environ.get("DVLA_DECODER_ALGEBRA", "1") != "0"
     _identical_cache = {}
 
     @staticmethod
@@ -130,12 +129,6 @@ class _WorldDecoder(nn.Module):
         B, S = feature.shape[:2]
         n = B * S * n_groups
         emb = projector(feature.reshape(-1, feature.shape[-1])).view(n, n_per, hidden)
-        if not _WorldDecoder.ALGEBRA or not all(isinstance(b.norm1, LayerNorm) for b in blocks):
-            mask_tokens = mask_token.expand(n, n_mask, -1)
-            x = torch.cat((emb, mask_tokens), dim=1) + pos_emb
-            x = blocks(x)
-            x = norm(x[:, -n_mask:, :].reshape(-1, hidden))
-            return pred(x, act=act)
         emb = emb + pos_emb[:, :n_per]
         if _WorldDecoder._mask_rows_identical(pos_emb, n_per):
             m = (mask_token + pos_emb[:, n_per:n_per + 1]).expand(n, 1, hidden)
@@ -502,7 +495,7 @@ class DreamVLA(nn.Module):
             parts.append(self.action_pred_token)
         return parts
 
-    FUSED_SAMPLER = os.environ.get("DVLA_DIT_FUSED", "1") != "0"
+    FUSED_SAMPLER = True
 
     def _ddim_actions(self, feat, sample_noise, dev):
         """10-step DDIM with classifier-free guidance 1.5 (:935-987) on feat [n, action_pred_steps, D] -> [n, steps, 7]."""

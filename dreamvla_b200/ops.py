@@ -9,8 +9,6 @@ into it in its epilogue and autograd receives None; 1-D parameters (biases, Laye
 """
 from __future__ import annotations
 
-import os
-
 import torch
 
 from . import _lib as L
@@ -169,14 +167,9 @@ def linear(x, weight, bias=None, *, act=None, residual=None, weight_kn=False, dr
                          float(dropout_p), float(alpha))
 
 
-# A/B switch: apply act'(pre) in the epilogue of the second layer's dgrad GEMM (DVLA_FUSE_ACT_BWD=1) instead of the separate
-# HBM-bound act_bwd kernel.
-_FUSE_ACT_BWD = os.environ.get("DVLA_FUSE_ACT_BWD", "0") == "1"
-
-
 class _MLP(torch.autograd.Function):
-    """y = dropout(act(x W1^T + b1) W2^T + b2) + residual with the activation backward fused into the dgrad GEMM of the
-    second layer (epilogue multiplies by act'(pre-activation)): no stand-alone elementwise pass in the backward."""
+    """y = dropout(act(x W1^T + b1) W2^T + b2) + residual.  The backward applies act'(pre-activation) to the second layer's
+    dgrad output in one elementwise pass, which also accumulates the first layer's bias gradient into its flat slot."""
 
     @staticmethod
     def forward(ctx, x, w1, b1, w2, b2, residual, act, weight_kn, dropout_p):
@@ -204,13 +197,9 @@ class _MLP(torch.autograd.Function):
         dy2 = _as2d(_bf16c(dy))
         d_res = dy.view(res_shape) if res_shape is not None and ctx.needs_input_grad[5] else None
         dz2 = L.dropout(dy2, dropout_p, seed, seed_ptr=seed_counter(dy2.device)) if dropout_p > 0 else dy2
-        # (dZ2 W2) * act'(pre).  The GEMM can apply act' in its epilogue (aux_in); the act' evaluation then sits on the
-        # GEMM's critical path, so the HBM-bound elementwise kernel is the default.
-        b1_done = False
-        if _FUSE_ACT_BWD:
-            dh = L.gemm(dz2, w2, b_mn=not weight_kn, aux_in=aux, act=act)
-        else:                                 # act' and the first layer's bias gradient in one pass over [rows, hidden]
-            dh, b1_done = _act_bwd_with_bias_grad(L.gemm(dz2, w2, b_mn=not weight_kn), aux, act, b1)
+        # (dZ2 W2) * act'(pre) in a separate pass: in the GEMM's epilogue (aux_in) the act' evaluation would sit on the
+        # GEMM's critical path
+        dh, b1_done = _act_bwd_with_bias_grad(L.gemm(dz2, w2, b_mn=not weight_kn), aux, act, b1)
         dw1 = dw2 = db1 = db2 = dx = None
         if w2.requires_grad:
             dw2 = _accum_grad_2d(w2, h, dz2, True, True) if weight_kn else _accum_grad_2d(w2, dz2, h, True, True)

@@ -1,5 +1,5 @@
 """Timing of the action sampler alone: fused megakernel (csrc/dit_sampler.cu) vs the module path, batch 1 and 2.
-   python tools/prof_sampler.py            (DVLA_DIT_CTAS=n varies the cooperative grid)"""
+   python tools/prof_sampler.py"""
 import os
 import sys
 
@@ -41,5 +41,5 @@ for bs in (1, 2):
                 run()
             e1.record()
             torch.cuda.synchronize()
-        print(f"sampler bs={bs} {'fused megakernel' if fused else 'module path (graph replay)'}: {e0.elapsed_time(e1) / 10:.3f} ms "
-              f"(DVLA_DIT_CTAS={os.environ.get('DVLA_DIT_CTAS', 'all')})", flush=True)
+        print(f"sampler bs={bs} {'fused megakernel' if fused else 'module path (graph replay)'}: {e0.elapsed_time(e1) / 10:.3f} ms",
+              flush=True)
