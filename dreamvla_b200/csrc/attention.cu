@@ -1072,6 +1072,7 @@ int attn_fwd_dispatch(const dvla_attn_fwd_args* a, cudaStream_t s) {
   if (a->H > 65535 || a->B > 65535) { set_error("attn_fwd: B,H must be <= 65535"); return DVLA_ERR_UNSUPPORTED; }
   if (a->mask && a->mask_words * 32 < a->Lk) { set_error("attn_fwd: mask_words too small"); return DVLA_ERR_INVALID; }
   if (a->mask && !a->tile_flags) { set_error("attn_fwd: mask given without tile_flags"); return DVLA_ERR_INVALID; }
+  if (!(a->dropout_p >= 0.f && a->dropout_p < 1.f)) { set_error("attn_fwd: dropout_p out of range [0, 1)"); return DVLA_ERR_INVALID; }
   if (a->key_bias) {
     if (!attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p)) {
       set_error("attn_fwd: key_bias needs the short-sequence kernels (Lq <= 32, Lk <= 64, no mask, no dropout)");
@@ -1130,6 +1131,7 @@ int attn_bwd_dispatch(const dvla_attn_bwd_args* a, cudaStream_t s) {
   if (!a->lse || !a->delta) { set_error("attn_bwd: lse/delta null"); return DVLA_ERR_INVALID; }
   if (a->B <= 0 || a->H <= 0 || a->Lq <= 0 || a->Lk <= 0) { set_error("attn_bwd: non-positive dims"); return DVLA_ERR_INVALID; }
   if (a->mask && !a->tile_flags) { set_error("attn_bwd: mask given without tile_flags"); return DVLA_ERR_INVALID; }
+  if (!(a->dropout_p >= 0.f && a->dropout_p < 1.f)) { set_error("attn_bwd: dropout_p out of range [0, 1)"); return DVLA_ERR_INVALID; }
   AttnParams p;
   memset(&p, 0, sizeof(p));
   p.q = (const bf16*)a->q; p.k = (const bf16*)a->k; p.v = (const bf16*)a->v; p.o = (const bf16*)a->o; p.d_o = (const bf16*)a->d_o;

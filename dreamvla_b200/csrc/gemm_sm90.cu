@@ -116,8 +116,8 @@ __device__ __forceinline__ void epilogue8(float (&v)[8], int row, int col, const
     act_fwd_n<8>(v, p.act);
   }
   if (p.drop_scale != 0.f) {
-    // element index = row*N + col; 8-element RNG blocks need col%8==0 alignment relative to row*N -> use (row*N+col)/8
-    // only when N%8==0, otherwise fall back to per-row block indexing (row*ceil(N/8) + col/8).
+    // RNG block = row*ceil(N/8) + col/8, bit col%8 (include/dvla.h; the same mask as dvla_dropout): each row starts a new
+    // block, so the mask of an element depends on its (row, col) only, never on the tiling.
     const uint64_t blk = static_cast<uint64_t>(row) * static_cast<uint64_t>((p.N + 7) >> 3) + (col >> 3);
     const uint64_t seed = p.drop_seed + (p.drop_seed_ptr ? __ldg(p.drop_seed_ptr) : 0ull);
     const uint32_t keep = dropout_keep8(seed, blk, p.drop_thresh);
@@ -793,7 +793,7 @@ int gemm_dispatch(const dvla_gemm_args* a, cudaStream_t stream) {
   if (!a || !a->a || !a->b || !a->out) { set_error("dvla_gemm: null pointer"); return DVLA_ERR_INVALID; }
   if (a->M <= 0 || a->N <= 0 || a->K <= 0) { set_error("dvla_gemm: non-positive dims M=%lld N=%lld K=%lld", (long long)a->M, (long long)a->N, (long long)a->K); return DVLA_ERR_INVALID; }
   if (a->aux_in && a->aux_out) { set_error("dvla_gemm: aux_in and aux_out are exclusive"); return DVLA_ERR_INVALID; }
-  if (a->dropout_p < 0.f || a->dropout_p >= 1.f) { set_error("dvla_gemm: dropout_p out of range"); return DVLA_ERR_INVALID; }
+  if (!(a->dropout_p >= 0.f && a->dropout_p < 1.f)) { set_error("dvla_gemm: dropout_p out of range"); return DVLA_ERR_INVALID; }
   GemmParams p;
   memset(&p, 0, sizeof(p));
   p.out = a->out; p.bias = (const bf16*)a->bias; p.residual = a->residual;

@@ -468,7 +468,7 @@ __global__ void dropout_kernel(const bf16* __restrict__ x, bf16* __restrict__ y,
 int dropout_dispatch(const void* x, void* y, int64_t rows, int64_t N, int64_t ldx, int64_t ldy, float p, uint64_t seed,
                      const uint64_t* seed_ptr, cudaStream_t s) {
   if (!x || !y) { set_error("dropout: null pointer"); return DVLA_ERR_INVALID; }
-  if (p < 0.f || p >= 1.f) { set_error("dropout: p out of range"); return DVLA_ERR_INVALID; }
+  if (!(p >= 0.f && p < 1.f)) { set_error("dropout: p out of range"); return DVLA_ERR_INVALID; }
   if (rows <= 0 || N <= 0) return DVLA_OK;
   const uint32_t thresh = (uint32_t)(p * 65536.0f + 0.5f);
   const float scale = 1.0f / (1.0f - (float)thresh / 65536.0f);

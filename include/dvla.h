@@ -61,7 +61,7 @@ typedef struct {
   int32_t act;
   int32_t out_fp32;
   float alpha;
-  float dropout_p;        /* 0 disables */
+  float dropout_p;        /* in [0, 1), anything else (NaN too) is DVLA_ERR_INVALID; 0 disables */
   uint64_t dropout_seed;  /* RNG block = m*ceil(N/8) + n/8, bit n%8 (same convention as dvla_dropout) */
   const uint64_t* dropout_seed_ptr; /* optional DEVICE counter added to dropout_seed at run time (CUDA-graph replays) */
   /* optional scratch of >= dvla_gemm_workspace_bytes() bytes, 16-byte aligned, owned by one stream (calls on one stream may
@@ -147,7 +147,8 @@ typedef struct {
   int64_t o_sb, o_ss, o_sh;
   int32_t mask_words;         /* uint32 words per mask row */
   float scale;
-  float dropout_p; uint64_t dropout_seed; /* attention-probability dropout (gpt2.py:272); RNG block = ((b*H+h)*Lq+i)*ceil(Lk/8)+j/8 */
+  float dropout_p; uint64_t dropout_seed; /* attention-probability dropout (gpt2.py:272), p in [0, 1) (else DVLA_ERR_INVALID);
+                                             RNG block = ((b*H+h)*Lq+i)*ceil(Lk/8)+j/8, bit j%8 */
   const uint64_t* dropout_seed_ptr;       /* optional device counter added to dropout_seed */
   const float* key_bias;      /* optional fp32 [Lk]: added to the scaled score of key j before the softmax (natural-log units).
                                  log(r) makes key j count r times -- the identical-mask-token form of a world decoder

@@ -19,7 +19,7 @@ def chk():
     return c
 
 
-@pytest.mark.parametrize("group", ["gemm_basic", "gemm_epilogue", "gemm_splitk", "gemm_tail", "norm", "attn", "loss"])
+@pytest.mark.parametrize("group", ["gemm_basic", "gemm_epilogue", "gemm_splitk", "gemm_tail", "norm", "attn", "loss", "act_bwd_colsum"])
 def test_kernel_group(chk, group):
     chk.RESULTS.clear()
     chk.GROUPS[group]()
