@@ -97,13 +97,48 @@ class DitSamplerArgs(C.Structure):
                 ("n_steps", _i64), ("cfg_scale", _f32), ("workspace", _vp), ("workspace_bytes", _i64)]
 
 
-EXPORTS = [
-    "dvla_version", "dvla_last_error", "dvla_launch_count", "dvla_gemm", "dvla_gemm_plan", "dvla_gemm_plan_unit", "dvla_layernorm_fwd", "dvla_layernorm_bwd",
-    "dvla_attn_fwd", "dvla_attn_bwd", "dvla_attn_mask_tiles", "dvla_colsum_accum", "dvla_accum_fp32_into_bf16",
-    "dvla_dropout", "dvla_act_bwd", "dvla_act_bwd_colsum", "dvla_cat_broadcast", "dvla_shift_crop", "dvla_resize_nearest", "dvla_image_fn", "dvla_bicubic_taps", "dvla_bicubic_coeffs", "dvla_mse_loss", "dvla_cosine_loss", "dvla_silog_stats", "dvla_silog_finish",
-    "dvla_sumsq", "dvla_adamw", "dvla_adamw_master", "dvla_grad_clip_scale", "dvla_attn_bwd_workspace_bytes", "dvla_silog_workspace_bytes",
-    "dvla_gemm_workspace_bytes", "dvla_set_sm_budget", "dvla_dit_ddim_sample", "dvla_dit_sampler_workspace_bytes",
-]
+# name -> (restype, argtypes) of every function include/dvla.h declares; tests/test_abi_cpu.py checks it against the header.
+# Pointers (device buffers, args structs, streams) are c_void_p: it takes tensor.data_ptr(), None and C.byref(...).
+_int = C.c_int
+PROTOTYPES = {
+    "dvla_version": (_int, []),
+    "dvla_last_error": (C.c_char_p, []),
+    "dvla_launch_count": (_i64, []),
+    "dvla_gemm": (_int, [_vp, _vp]),
+    "dvla_gemm_plan": (_int, [_vp, _vp]),
+    "dvla_gemm_plan_unit": (_int, [_vp, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "dvla_layernorm_fwd": (_int, [_vp, _vp]),
+    "dvla_layernorm_bwd": (_int, [_vp, _vp]),
+    "dvla_attn_fwd": (_int, [_vp, _vp]),
+    "dvla_attn_bwd": (_int, [_vp, _vp]),
+    "dvla_attn_mask_tiles": (_int, [_vp, _i32, _i64, _i64, _vp, _vp]),
+    "dvla_colsum_accum": (_int, [_vp, _i64, _i64, _i64, _vp, _vp]),
+    "dvla_accum_fp32_into_bf16": (_int, [_vp, _vp, _i64, _vp]),
+    "dvla_dropout": (_int, [_vp, _vp, _i64, _i64, _i64, _i64, _f32, _u64, _vp, _vp]),
+    "dvla_cat_broadcast": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _i64, _vp]),
+    "dvla_act_bwd": (_int, [_vp, _vp, _vp, _i64, _i32, _vp]),
+    "dvla_act_bwd_colsum": (_int, [_vp, _vp, _vp, _i64, _i64, _i32, _vp, _vp]),
+    "dvla_mse_loss": (_int, [_vp, _vp, _vp, _i64, _i64, _f32, _vp, _vp, _vp]),
+    "dvla_cosine_loss": (_int, [_vp, _vp, _i64, _i64, _f32, _vp, _vp, _vp]),
+    "dvla_silog_stats": (_int, [_vp, _vp, _i64, _vp, _vp]),
+    "dvla_silog_finish": (_int, [_vp, _vp, _i64, _vp, _f32, _f32, _vp, _vp, _vp]),
+    "dvla_sumsq": (_int, [_vp, _i64, _vp, _vp]),
+    "dvla_adamw": (_int, [_vp, _vp]),
+    "dvla_adamw_master": (_int, [_vp, _vp]),
+    "dvla_grad_clip_scale": (_int, [_vp, _i64, _vp, _f32, _f32, _vp]),
+    "dvla_dit_sampler_workspace_bytes": (_i64, [_i64, _i64, _i64, _i64, _i64]),
+    "dvla_dit_ddim_sample": (_int, [_vp, _vp]),
+    "dvla_shift_crop": (_int, [_vp, _vp, _vp, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _vp]),
+    "dvla_resize_nearest": (_int, [_vp, _vp, _i64, _i64, _i64, _i64, _i64, _i32, _vp]),
+    "dvla_image_fn": (_int, [_vp, _vp]),
+    "dvla_bicubic_taps": (_i32, [_i64, _i64]),
+    "dvla_bicubic_coeffs": (_int, [_i64, _i64, _i64, _i64, _vp, _vp]),
+    "dvla_set_sm_budget": (_int, [_int]),
+    "dvla_attn_bwd_workspace_bytes": (_i64, [_i64, _i64, _i64]),
+    "dvla_silog_workspace_bytes": (_i64, []),
+    "dvla_gemm_workspace_bytes": (_i64, [_vp]),
+}
+EXPORTS = sorted(PROTOTYPES)
 
 _lib = None
 
@@ -118,14 +153,11 @@ def load() -> C.CDLL:
             f"{LIB_PATH} not found: build it with `python -m dreamvla_b200.build` (nvcc, sm_90a). "
             "dreamvla_b200 has no CPU or PyTorch fallback for its kernels.")
     lib = C.CDLL(LIB_PATH)
-    lib.dvla_last_error.restype = C.c_char_p
-    lib.dvla_launch_count.restype = C.c_int64
-    for name in EXPORTS:
+    for name, (restype, argtypes) in PROTOTYPES.items():
         if not hasattr(lib, name):
             raise RuntimeError(f"{LIB_PATH} does not export {name} (stale build? run `python -m dreamvla_b200.build`)")
-    for name in ("dvla_attn_bwd_workspace_bytes", "dvla_silog_workspace_bytes", "dvla_gemm_workspace_bytes",
-                 "dvla_dit_sampler_workspace_bytes"):
-        getattr(lib, name).restype = C.c_int64
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = restype, argtypes
     _lib = lib
     return lib
 
@@ -134,13 +166,17 @@ def launch_count() -> int:
     return int(load().dvla_launch_count())
 
 
-def _check(rc: int, what: str) -> None:
-    if rc != 0:
-        raise RuntimeError(f"{what} failed ({rc}): {load().dvla_last_error().decode()}")
+def _call(name: str, *args) -> int:
+    """Calls library function `name` and returns its result; a negative dvla_status raises RuntimeError with the text of
+    dvla_last_error()."""
+    rc = getattr(load(), name)(*args)
+    if rc < 0:
+        raise RuntimeError(f"{name} failed ({rc}): {load().dvla_last_error().decode()}")
+    return rc
 
 
-def _stream() -> C.c_void_p:
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+def _stream() -> int:
+    return torch.cuda.current_stream().cuda_stream
 
 
 def _ptr(t) -> int | None:
@@ -210,7 +246,7 @@ def gemm(a, b, *, a_mn=False, b_mn=False, bias=None, act=0, residual=None, aux_o
     args.dropout_seed_ptr = _ptr(dropout_seed_ptr)
     ws = gemm_workspace(a.device)
     args.workspace, args.workspace_bytes = ws.data_ptr(), ws.numel()
-    _check(load().dvla_gemm(C.byref(args), _stream()), "dvla_gemm")
+    _call("dvla_gemm", C.byref(args), _stream())
     return out
 
 
@@ -223,7 +259,7 @@ def layernorm_fwd(x2d, gamma, beta, eps, save_stats=True):
     rstd = torch.empty(rows, device=x2d.device, dtype=torch.float32) if save_stats else None
     a = LayerNormFwdArgs(x2d.data_ptr(), _ptr(gamma), _ptr(beta), y.data_ptr(), _ptr(mean), _ptr(rstd), rows, D,
                          x2d.stride(0), y.stride(0), float(eps))
-    _check(load().dvla_layernorm_fwd(C.byref(a), _stream()), "dvla_layernorm_fwd")
+    _call("dvla_layernorm_fwd", C.byref(a), _stream())
     return y, mean, rstd
 
 
@@ -235,7 +271,7 @@ def layernorm_bwd(dy2d, x2d, gamma, mean, rstd, dgamma_f32, dbeta_f32, dres2d=No
     dx = torch.empty_like(x2d)
     a = LayerNormBwdArgs(dy2d.data_ptr(), x2d.data_ptr(), _ptr(gamma), mean.data_ptr(), rstd.data_ptr(), dx.data_ptr(),
                          _ptr(dgamma_f32), _ptr(dbeta_f32), rows, D, D, _ptr(dres2d))
-    _check(load().dvla_layernorm_bwd(C.byref(a), _stream()), "dvla_layernorm_bwd")
+    _call("dvla_layernorm_bwd", C.byref(a), _stream())
     return dx
 
 
@@ -267,7 +303,7 @@ def attn_fwd(q, k, v, scale, mask_bits=None, tile_flags=None, dropout_p=0.0, dro
     if key_bias is not None:
         assert key_bias.dtype == torch.float32 and key_bias.is_contiguous() and key_bias.numel() == Lk
         a.key_bias = key_bias.data_ptr()
-    _check(load().dvla_attn_fwd(C.byref(a), _stream()), "dvla_attn_fwd")
+    _call("dvla_attn_fwd", C.byref(a), _stream())
     return o, lse
 
 
@@ -275,7 +311,7 @@ def attn_bwd(q, k, v, o, d_o, lse, scale, dq, dk, dv, mask_bits=None, tile_flags
              dropout_seed_ptr=None, key_bias=None):
     B, Lq, H, _ = q.shape
     Lk = k.shape[1]
-    ws = int(load().dvla_attn_bwd_workspace_bytes(_i64(B), _i64(H), _i64(Lq)))
+    ws = load().dvla_attn_bwd_workspace_bytes(B, H, Lq)
     delta = torch.empty(ws // 4, device=q.device, dtype=torch.float32)
     a = AttnBwdArgs()
     a.q, a.k, a.v, a.o, a.d_o = q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), d_o.data_ptr()
@@ -295,37 +331,33 @@ def attn_bwd(q, k, v, o, d_o, lse, scale, dq, dk, dv, mask_bits=None, tile_flags
     a.scale, a.dropout_p, a.dropout_seed = float(scale), float(dropout_p), int(dropout_seed)
     a.dropout_seed_ptr = _ptr(dropout_seed_ptr)
     a.key_bias = _ptr(key_bias)
-    _check(load().dvla_attn_bwd(C.byref(a), _stream()), "dvla_attn_bwd")
+    _call("dvla_attn_bwd", C.byref(a), _stream())
 
 
 def attn_mask_tiles(mask_bits, Lq, Lk):
     nqt, nkt = (Lq + 63) // 64, (Lk + 63) // 64
     flags = torch.empty((nqt, nkt), device=mask_bits.device, dtype=torch.uint8)
-    _check(load().dvla_attn_mask_tiles(C.c_void_p(mask_bits.data_ptr()), C.c_int32(mask_bits.shape[1]), _i64(Lq),
-                                       _i64(Lk), C.c_void_p(flags.data_ptr()), _stream()), "dvla_attn_mask_tiles")
+    _call("dvla_attn_mask_tiles", mask_bits.data_ptr(), mask_bits.shape[1], Lq, Lk, flags.data_ptr(), _stream())
     return flags
 
 
 def colsum_accum(x2d, out_f32):
     rows, N = x2d.shape
     assert x2d.stride(1) == 1
-    _check(load().dvla_colsum_accum(C.c_void_p(x2d.data_ptr()), _i64(rows), _i64(N), _i64(x2d.stride(0)),
-                                    C.c_void_p(out_f32.data_ptr()), _stream()), "dvla_colsum_accum")
+    _call("dvla_colsum_accum", x2d.data_ptr(), rows, N, x2d.stride(0), out_f32.data_ptr(), _stream())
 
 
 def accum_fp32_into_bf16(src_f32, dst_bf16):
     assert src_f32.is_contiguous() and dst_bf16.is_contiguous() and src_f32.numel() == dst_bf16.numel()
-    _check(load().dvla_accum_fp32_into_bf16(C.c_void_p(src_f32.data_ptr()), C.c_void_p(dst_bf16.data_ptr()),
-                                            _i64(src_f32.numel()), _stream()), "dvla_accum_fp32_into_bf16")
+    _call("dvla_accum_fp32_into_bf16", src_f32.data_ptr(), dst_bf16.data_ptr(), src_f32.numel(), _stream())
 
 
 def dropout(x2d, p, seed, out=None, seed_ptr=None):
     rows, N = x2d.shape
     assert x2d.stride(1) == 1
     y = torch.empty((rows, N), device=x2d.device, dtype=torch.bfloat16) if out is None else out
-    _check(load().dvla_dropout(C.c_void_p(x2d.data_ptr()), C.c_void_p(y.data_ptr()), _i64(rows), _i64(N),
-                               _i64(x2d.stride(0)), _i64(y.stride(0)), _f32(p), _u64(seed), C.c_void_p(_ptr(seed_ptr)),
-                               _stream()), "dvla_dropout")
+    _call("dvla_dropout", x2d.data_ptr(), y.data_ptr(), rows, N, x2d.stride(0), y.stride(0), p, seed, _ptr(seed_ptr),
+          _stream())
     return y
 
 
@@ -340,9 +372,8 @@ def shift_crop(x, shifts_xy, pad, out_dtype=None):
     n, c, h, w = x.shape
     assert shifts_xy.dtype == torch.int32 and shifts_xy.shape == (n, 2) and shifts_xy.is_contiguous()
     out = torch.empty_like(x, dtype=out_dtype or x.dtype)
-    _check(load().dvla_shift_crop(C.c_void_p(x.data_ptr()), C.c_void_p(out.data_ptr()), C.c_void_p(shifts_xy.data_ptr()), _i64(n),
-                                  _i64(c), _i64(h), _i64(w), C.c_int32(int(pad)), C.c_int32(_DT[x.dtype]),
-                                  C.c_int32(_DT[out.dtype]), _stream()), "dvla_shift_crop")
+    _call("dvla_shift_crop", x.data_ptr(), out.data_ptr(), shifts_xy.data_ptr(), n, c, h, w, int(pad), _DT[x.dtype],
+          _DT[out.dtype], _stream())
     return out
 
 
@@ -353,8 +384,7 @@ def resize_nearest(x, hout, wout, out_dtype=torch.float32):
     hin, win = x.shape[-2:]
     n = x.numel() // (hin * win)
     out = torch.empty((*x.shape[:-2], hout, wout), device=x.device, dtype=out_dtype)
-    _check(load().dvla_resize_nearest(C.c_void_p(x.data_ptr()), C.c_void_p(out.data_ptr()), _i64(n), _i64(hin), _i64(win),
-                                      _i64(hout), _i64(wout), C.c_int32(_DT[out_dtype]), _stream()), "dvla_resize_nearest")
+    _call("dvla_resize_nearest", x.data_ptr(), out.data_ptr(), n, hin, win, hout, wout, _DT[out_dtype], _stream())
     return out
 
 
@@ -373,13 +403,10 @@ def image_fn_geometry(h, w, size=IMAGE_FN_SIZE):
 def bicubic_coeffs(in_size, out_size, first, count):
     """Pillow's bicubic bounds / int32 coefficients of outputs [first, first + count) of a line resized from in_size to
     out_size (host only, no GPU): (bounds int32 [count, 2] = (first input pixel, taps used), coeffs int32 [count, taps])."""
-    lib = load()
-    taps = int(lib.dvla_bicubic_taps(_i64(in_size), _i64(out_size)))
-    _check(min(taps, 0), "dvla_bicubic_taps")
+    taps = _call("dvla_bicubic_taps", in_size, out_size)
     bounds = torch.zeros((count, 2), dtype=torch.int32)
     coeffs = torch.zeros((count, taps), dtype=torch.int32)
-    _check(lib.dvla_bicubic_coeffs(_i64(in_size), _i64(out_size), _i64(first), _i64(count), C.c_void_p(bounds.data_ptr()),
-                                   C.c_void_p(coeffs.data_ptr())), "dvla_bicubic_coeffs")
+    _call("dvla_bicubic_coeffs", in_size, out_size, first, count, bounds.data_ptr(), coeffs.data_ptr())
     return bounds, coeffs
 
 
@@ -413,7 +440,7 @@ def image_fn(frames, lut, out_dtype=torch.float32, flip_vertical=False):
     xb, xc, yb, yc = image_fn_tables(h, w, frames.device)
     a = ImageFnArgs(frames.data_ptr(), out.data_ptr(), n, h, w, c, xb.data_ptr(), xc.data_ptr(), yb.data_ptr(), yc.data_ptr(),
                     lut.data_ptr(), int(bool(flip_vertical)), _DT[out_dtype])
-    _check(load().dvla_image_fn(C.byref(a), _stream()), "dvla_image_fn")
+    _call("dvla_image_fn", C.byref(a), _stream())
     return out
 
 
@@ -424,53 +451,45 @@ def act_bwd(dy, pre, act, colsum_out=None):
     if colsum_out is not None:
         N = dy.shape[-1]
         assert colsum_out.dtype == torch.float32 and colsum_out.numel() == N and colsum_out.is_contiguous()
-        _check(load().dvla_act_bwd_colsum(C.c_void_p(dy.data_ptr()), C.c_void_p(pre.data_ptr()), C.c_void_p(dx.data_ptr()),
-                                          _i64(dy.numel() // N), _i64(N), C.c_int32(act), C.c_void_p(colsum_out.data_ptr()),
-                                          _stream()), "dvla_act_bwd_colsum")
+        _call("dvla_act_bwd_colsum", dy.data_ptr(), pre.data_ptr(), dx.data_ptr(), dy.numel() // N, N, act,
+              colsum_out.data_ptr(), _stream())
         return dx
-    _check(load().dvla_act_bwd(C.c_void_p(dy.data_ptr()), C.c_void_p(pre.data_ptr()), C.c_void_p(dx.data_ptr()),
-                               _i64(dy.numel()), C.c_int32(act), _stream()), "dvla_act_bwd")
+    _call("dvla_act_bwd", dy.data_ptr(), pre.data_ptr(), dx.data_ptr(), dy.numel(), act, _stream())
     return dx
 
 
 def mse_loss(pred2d, label2d, row_mask, weight, loss_out, dpred):
     rows, Cc = pred2d.shape
     assert pred2d.is_contiguous() and label2d.is_contiguous()
-    _check(load().dvla_mse_loss(C.c_void_p(pred2d.data_ptr()), C.c_void_p(label2d.data_ptr()),
-                                C.c_void_p(_ptr(row_mask)), _i64(rows), _i64(Cc), _f32(weight),
-                                C.c_void_p(loss_out.data_ptr()), C.c_void_p(_ptr(dpred)), _stream()), "dvla_mse_loss")
+    _call("dvla_mse_loss", pred2d.data_ptr(), label2d.data_ptr(), _ptr(row_mask), rows, Cc, weight, loss_out.data_ptr(),
+          _ptr(dpred), _stream())
 
 
 def cosine_loss(pred2d, label2d, weight, loss_out, dpred):
     rows, Cc = pred2d.shape
     assert pred2d.is_contiguous() and label2d.is_contiguous()
-    _check(load().dvla_cosine_loss(C.c_void_p(pred2d.data_ptr()), C.c_void_p(label2d.data_ptr()), _i64(rows), _i64(Cc),
-                                   _f32(weight), C.c_void_p(loss_out.data_ptr()), C.c_void_p(_ptr(dpred)), _stream()),
-           "dvla_cosine_loss")
+    _call("dvla_cosine_loss", pred2d.data_ptr(), label2d.data_ptr(), rows, Cc, weight, loss_out.data_ptr(), _ptr(dpred),
+          _stream())
 
 
 def silog_loss(pred, label, lambd, weight, loss_out, dpred):
     assert pred.is_contiguous() and label.is_contiguous()
     n = pred.numel()
-    stats = torch.zeros(int(load().dvla_silog_workspace_bytes()) // 4, device=pred.device, dtype=torch.float32)
-    _check(load().dvla_silog_stats(C.c_void_p(pred.data_ptr()), C.c_void_p(label.data_ptr()), _i64(n),
-                                   C.c_void_p(stats.data_ptr()), _stream()), "dvla_silog_stats")
-    _check(load().dvla_silog_finish(C.c_void_p(pred.data_ptr()), C.c_void_p(label.data_ptr()), _i64(n),
-                                    C.c_void_p(stats.data_ptr()), _f32(lambd), _f32(weight),
-                                    C.c_void_p(loss_out.data_ptr()), C.c_void_p(_ptr(dpred)), _stream()),
-           "dvla_silog_finish")
+    stats = torch.zeros(load().dvla_silog_workspace_bytes() // 4, device=pred.device, dtype=torch.float32)
+    _call("dvla_silog_stats", pred.data_ptr(), label.data_ptr(), n, stats.data_ptr(), _stream())
+    _call("dvla_silog_finish", pred.data_ptr(), label.data_ptr(), n, stats.data_ptr(), lambd, weight, loss_out.data_ptr(),
+          _ptr(dpred), _stream())
 
 
 def sumsq(g_bf16, out_f32):
-    _check(load().dvla_sumsq(C.c_void_p(g_bf16.data_ptr()), _i64(g_bf16.numel()), C.c_void_p(out_f32.data_ptr()),
-                             _stream()), "dvla_sumsq")
+    _call("dvla_sumsq", g_bf16.data_ptr(), g_bf16.numel(), out_f32.data_ptr(), _stream())
 
 
 def adamw(p, g, m, v, *, sumsq_t, lr_t, step_t, beta1, beta2, eps, weight_decay, max_norm, grad_scale=1.0,
           zero_grad=True):
     a = AdamWArgs(p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), p.numel(), _ptr(sumsq_t), lr_t.data_ptr(),
                   step_t.data_ptr(), beta1, beta2, eps, weight_decay, max_norm, grad_scale, int(zero_grad))
-    _check(load().dvla_adamw(C.byref(a), _stream()), "dvla_adamw")
+    _call("dvla_adamw", C.byref(a), _stream())
 
 
 def adamw_master(p32, p, g, m, v, *, sumsq_t, lr_t, step_t, beta1, beta2, eps, weight_decay, max_norm, grad_scale=1.0,
@@ -481,18 +500,17 @@ def adamw_master(p32, p, g, m, v, *, sumsq_t, lr_t, step_t, beta1, beta2, eps, w
     a = AdamWMasterArgs(p32.data_ptr(), p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), p32.numel(), _ptr(sumsq_t),
                         lr_t.data_ptr(), step_t.data_ptr(), beta1, beta2, eps, weight_decay, max_norm, grad_scale,
                         int(zero_grad))
-    _check(load().dvla_adamw_master(C.byref(a), _stream()), "dvla_adamw_master")
+    _call("dvla_adamw_master", C.byref(a), _stream())
 
 
 def grad_clip_scale(g, sumsq_t, max_norm, grad_scale=1.0):
     """g *= grad_scale * min(1, max_norm / (sqrt(sumsq) * grad_scale + 1e-6)) in place (clip_grad_norm_ on the flat buffer)."""
-    _check(load().dvla_grad_clip_scale(C.c_void_p(g.data_ptr()), _i64(g.numel()), C.c_void_p(sumsq_t.data_ptr()),
-                                       _f32(max_norm), _f32(grad_scale), _stream()), "dvla_grad_clip_scale")
+    _call("dvla_grad_clip_scale", g.data_ptr(), g.numel(), sumsq_t.data_ptr(), max_norm, grad_scale, _stream())
 
 
 def set_sm_budget(n_sms: int) -> int:
     """SMs the persistent GEMM kernels size their grids for (0 = all); returns the previous value."""
-    return int(load().dvla_set_sm_budget(C.c_int(int(n_sms))))
+    return load().dvla_set_sm_budget(int(n_sms))
 
 
 def cat_broadcast(e, m):
@@ -502,8 +520,7 @@ def cat_broadcast(e, m):
     b = m.shape[0]
     assert e.is_contiguous() and m.is_contiguous() and m.shape[1] == Cc and e.dtype == m.dtype == torch.bfloat16
     out = torch.empty((n, a + b, Cc), device=e.device, dtype=torch.bfloat16)
-    _check(load().dvla_cat_broadcast(C.c_void_p(e.data_ptr()), C.c_void_p(m.data_ptr()), C.c_void_p(out.data_ptr()), _i64(n),
-                                     _i64(a), _i64(b), _i64(Cc), _stream()), "dvla_cat_broadcast")
+    _call("dvla_cat_broadcast", e.data_ptr(), m.data_ptr(), out.data_ptr(), n, a, b, Cc, _stream())
     return out
 
 
@@ -524,7 +541,7 @@ def dit_ddim_sample(net, diffusion, z, noise, cfg_scale):
     z = z.contiguous()
     noise = noise.contiguous().float()
     out = torch.empty((bs, T, Cc), device=z.device, dtype=torch.float32)
-    ws_bytes = int(load().dvla_dit_sampler_workspace_bytes(_i64(bs), _i64(T), _i64(H), _i64(mlp), _i64(n_steps)))
+    ws_bytes = load().dvla_dit_sampler_workspace_bytes(bs, T, H, mlp, n_steps)
     ws = torch.empty(ws_bytes, device=z.device, dtype=torch.uint8)
     tmap = (_i32 * n_steps)(*[int(t) for t in diffusion.timestep_map])
     f32arr = lambda a: (_f32 * n_steps)(*[float(v) for v in a])     # noqa: E731
@@ -545,5 +562,5 @@ def dit_ddim_sample(net, diffusion, z, noise, cfg_scale):
     a.alphas_cumprod_prev = f32arr(diffusion.alphas_cumprod_prev)
     a.n_steps, a.cfg_scale = n_steps, float(cfg_scale)
     a.workspace, a.workspace_bytes = ws.data_ptr(), ws_bytes
-    _check(load().dvla_dit_ddim_sample(C.byref(a), _stream()), "dvla_dit_ddim_sample")
+    _call("dvla_dit_ddim_sample", C.byref(a), _stream())
     return out

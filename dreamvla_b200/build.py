@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libdvla_sm90.so")
-SOURCES = ["gemm_sm90.cu", "attention.cu", "attention_small.cu", "norm_act.cu", "loss_optim.cu", "dit_sampler.cu", "augment.cu", "capi.cu"]
+SOURCES = ["gemm_sm90.cu", "attention.cu", "attention_small.cu", "norm_act.cu", "loss_optim.cu", "dit_sampler.cu", "augment.cu", "state.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",

@@ -16,12 +16,10 @@
 #include <mutex>
 
 #include "common.cuh"
+#include "host.cuh"
 #include "../../include/dvla.h"
 
 namespace dvla {
-void set_error(const char* fmt, ...);
-void count_launch();
-int num_sms();
 
 constexpr float LOG2E = 1.4426950408889634f;
 constexpr float LN2 = 0.6931471805599453f;
@@ -997,31 +995,19 @@ __global__ void attn_mask_tiles_kernel(const uint32_t* __restrict__ mask, int ma
 }
 
 // ===================================================== host =======================================================
-#define DVLA_CHECK_LAUNCH(name)                                                                 \
-  do {                                                                                          \
-    cudaError_t e__ = cudaGetLastError();                                                       \
-    if (e__ != cudaSuccess) { set_error("%s launch: %s", name, cudaGetErrorString(e__)); return DVLA_ERR_CUDA; } \
-    count_launch();                                                                             \
-  } while (0)
-
 static bool strides_ok(const void* ptr, long long sb, long long ss, long long sh) {
   return ptr && (reinterpret_cast<uintptr_t>(ptr) % 16 == 0) && sb % 8 == 0 && ss % 8 == 0 && sh % 8 == 0;
 }
 
 bool attn_small_applicable(int64_t Lq, int64_t Lk, const void* mask, float dropout_p);   // attention_small.cu
-int attn_small_fwd_dispatch(const dvla_attn_fwd_args* a, cudaStream_t s);
-int attn_small_bwd_dispatch(const dvla_attn_bwd_args* a, cudaStream_t s);
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn get_encode_fn_shared();   // gemm_sm90.cu
+int attn_small_fwd(const dvla_attn_fwd_args* a, cudaStream_t s);
+int attn_small_bwd(const dvla_attn_bwd_args* a, cudaStream_t s);
 
 // [B, L, H, 64] strided view -> 4-D tensor map with 64 x 64 boxes, 128-byte swizzle (the layout the wgmma descriptors
 // expect); seq and head dims are ordered so that the strides ascend.
 static bool make_attn_tmap(CUtensorMap* out, const void* base, long long L, long long H, long long B, long long ss,
                            long long sh, long long sb, int* head_inner) {
-  EncodeTiledFn fn = get_encode_fn_shared();
+  EncodeTiledFn fn = get_encode_fn();
   if (!fn) { set_error("cuTensorMapEncodeTiled entry point not found"); return false; }
   *head_inner = (sh <= ss) ? 1 : 0;
   cuuint64_t dims[4]; cuuint64_t strides[3]; cuuint32_t box[4]; cuuint32_t estr[4] = {1, 1, 1, 1};
@@ -1061,52 +1047,6 @@ static int attn_fwd_wgmma_launch(const dvla_attn_fwd_args* a, const AttnParams& 
   return DVLA_OK;
 }
 
-int attn_fwd_dispatch(const dvla_attn_fwd_args* a, cudaStream_t s) {
-  if (!a) { set_error("attn_fwd: null args"); return DVLA_ERR_INVALID; }
-  if (!strides_ok(a->q, a->q_sb, a->q_ss, a->q_sh) || !strides_ok(a->k, a->k_sb, a->k_ss, a->k_sh) ||
-      !strides_ok(a->v, a->v_sb, a->v_ss, a->v_sh) || !strides_ok(a->o, a->o_sb, a->o_ss, a->o_sh)) {
-    set_error("attn_fwd: q/k/v/o must be non-null, 16-byte aligned with strides multiple of 8 elements");
-    return DVLA_ERR_INVALID;
-  }
-  if (a->B <= 0 || a->H <= 0 || a->Lq <= 0 || a->Lk <= 0) { set_error("attn_fwd: non-positive dims"); return DVLA_ERR_INVALID; }
-  if (a->H > 65535 || a->B > 65535) { set_error("attn_fwd: B,H must be <= 65535"); return DVLA_ERR_UNSUPPORTED; }
-  if (a->mask && a->mask_words * 32 < a->Lk) { set_error("attn_fwd: mask_words too small"); return DVLA_ERR_INVALID; }
-  if (a->mask && !a->tile_flags) { set_error("attn_fwd: mask given without tile_flags"); return DVLA_ERR_INVALID; }
-  if (!(a->dropout_p >= 0.f && a->dropout_p < 1.f)) { set_error("attn_fwd: dropout_p out of range [0, 1)"); return DVLA_ERR_INVALID; }
-  if (a->key_bias) {
-    if (!attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p)) {
-      set_error("attn_fwd: key_bias needs the short-sequence kernels (Lq <= 32, Lk <= 64, no mask, no dropout)");
-      return DVLA_ERR_UNSUPPORTED;
-    }
-    return attn_small_fwd_dispatch(a, s);
-  }
-  if (attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p))
-    return attn_small_fwd_dispatch(a, s);
-  AttnParams p;
-  memset(&p, 0, sizeof(p));
-  p.q = (const bf16*)a->q; p.k = (const bf16*)a->k; p.v = (const bf16*)a->v; p.out = (bf16*)a->o; p.lse = a->lse;
-  p.mask = a->mask; p.tile_flags = a->mask ? a->tile_flags : nullptr;
-  p.B = (int)a->B; p.H = (int)a->H; p.Lq = (int)a->Lq; p.Lk = (int)a->Lk;
-  p.nqt = (p.Lq + 63) / 64; p.nkt = (p.Lk + 63) / 64; p.mask_words = a->mask_words;
-  p.q_sb = a->q_sb; p.q_ss = a->q_ss; p.q_sh = a->q_sh; p.k_sb = a->k_sb; p.k_ss = a->k_ss; p.k_sh = a->k_sh;
-  p.v_sb = a->v_sb; p.v_ss = a->v_ss; p.v_sh = a->v_sh; p.o_sb = a->o_sb; p.o_ss = a->o_ss; p.o_sh = a->o_sh;
-  p.scale = a->scale;
-  if (a->dropout_p > 0.f) {
-    p.drop_thresh = (uint32_t)(a->dropout_p * 65536.0f + 0.5f);
-    p.drop_scale = 1.0f / (1.0f - (float)p.drop_thresh / 65536.0f);
-    p.drop_seed = a->dropout_seed;
-    p.drop_seed_ptr = a->dropout_seed_ptr;
-  }
-  // wgmma + TMA for the long sequences (backbone, ViT, decoders); the mma.sync kernel for short query blocks and strides a
-  // tensor map cannot express
-  if (a->Lq >= 96 && tmap_strides_ok(a->Lq, a->H, a->B, a->q_ss, a->q_sh, a->q_sb) &&
-      tmap_strides_ok(a->Lk, a->H, a->B, a->k_ss, a->k_sh, a->k_sb) && tmap_strides_ok(a->Lk, a->H, a->B, a->v_ss, a->v_sh, a->v_sb))
-    return attn_fwd_wgmma_launch(a, p, s);
-  attn_fwd_kernel<<<dim3(p.nqt, p.H, p.B), 128, 0, s>>>(p);
-  DVLA_CHECK_LAUNCH("attn_fwd");
-  return DVLA_OK;
-}
-
 template <bool DKV>
 static int attn_bwd_wgmma_launch(const WgmmaBwdMaps& tm, const AttnParams& p, cudaStream_t s) {
   static std::once_flag once;
@@ -1119,7 +1059,66 @@ static int attn_bwd_wgmma_launch(const WgmmaBwdMaps& tm, const AttnParams& p, cu
   return DVLA_OK;
 }
 
-int attn_bwd_dispatch(const dvla_attn_bwd_args* a, cudaStream_t s) {
+// The AttnParams fields the forward and backward share: operands q/k/v, o and lse, dims, tile counts, mask and dropout.
+template <class Args>
+static AttnParams attn_params(const Args* a) {
+  AttnParams p;
+  memset(&p, 0, sizeof(p));
+  p.q = (const bf16*)a->q; p.k = (const bf16*)a->k; p.v = (const bf16*)a->v; p.lse = const_cast<float*>(a->lse);
+  p.mask = a->mask; p.tile_flags = a->mask ? a->tile_flags : nullptr;
+  p.B = (int)a->B; p.H = (int)a->H; p.Lq = (int)a->Lq; p.Lk = (int)a->Lk;
+  p.nqt = (p.Lq + 63) / 64; p.nkt = (p.Lk + 63) / 64; p.mask_words = a->mask_words;
+  p.q_sb = a->q_sb; p.q_ss = a->q_ss; p.q_sh = a->q_sh; p.k_sb = a->k_sb; p.k_ss = a->k_ss; p.k_sh = a->k_sh;
+  p.v_sb = a->v_sb; p.v_ss = a->v_ss; p.v_sh = a->v_sh; p.o_sb = a->o_sb; p.o_ss = a->o_ss; p.o_sh = a->o_sh;
+  p.scale = a->scale;
+  if (a->dropout_p > 0.f) {
+    dropout_thresh_scale(a->dropout_p, &p.drop_thresh, &p.drop_scale);
+    p.drop_seed = a->dropout_seed;
+    p.drop_seed_ptr = a->dropout_seed_ptr;
+  }
+  return p;
+}
+
+}  // namespace dvla
+
+using namespace dvla;
+
+extern "C" int dvla_attn_fwd(const dvla_attn_fwd_args* a, void* stream) {
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  if (!a) { set_error("attn_fwd: null args"); return DVLA_ERR_INVALID; }
+  if (!strides_ok(a->q, a->q_sb, a->q_ss, a->q_sh) || !strides_ok(a->k, a->k_sb, a->k_ss, a->k_sh) ||
+      !strides_ok(a->v, a->v_sb, a->v_ss, a->v_sh) || !strides_ok(a->o, a->o_sb, a->o_ss, a->o_sh)) {
+    set_error("attn_fwd: q/k/v/o must be non-null, 16-byte aligned with strides multiple of 8 elements");
+    return DVLA_ERR_INVALID;
+  }
+  if (a->B <= 0 || a->H <= 0 || a->Lq <= 0 || a->Lk <= 0) { set_error("attn_fwd: non-positive dims"); return DVLA_ERR_INVALID; }
+  if (a->H > 65535 || a->B > 65535) { set_error("attn_fwd: B,H must be <= 65535"); return DVLA_ERR_UNSUPPORTED; }
+  if (a->mask && a->mask_words * 32 < a->Lk) { set_error("attn_fwd: mask_words too small"); return DVLA_ERR_INVALID; }
+  if (a->mask && !a->tile_flags) { set_error("attn_fwd: mask given without tile_flags"); return DVLA_ERR_INVALID; }
+  if (!dropout_rate_ok(a->dropout_p)) { set_error("attn_fwd: dropout_p out of range [0, 1)"); return DVLA_ERR_INVALID; }
+  if (a->key_bias) {
+    if (!attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p)) {
+      set_error("attn_fwd: key_bias needs the short-sequence kernels (Lq <= 32, Lk <= 64, no mask, no dropout)");
+      return DVLA_ERR_UNSUPPORTED;
+    }
+    return attn_small_fwd(a, s);
+  }
+  if (attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p))
+    return attn_small_fwd(a, s);
+  AttnParams p = attn_params(a);
+  p.out = (bf16*)a->o;
+  // wgmma + TMA for the long sequences (backbone, ViT, decoders); the mma.sync kernel for short query blocks and strides a
+  // tensor map cannot express
+  if (a->Lq >= 96 && tmap_strides_ok(a->Lq, a->H, a->B, a->q_ss, a->q_sh, a->q_sb) &&
+      tmap_strides_ok(a->Lk, a->H, a->B, a->k_ss, a->k_sh, a->k_sb) && tmap_strides_ok(a->Lk, a->H, a->B, a->v_ss, a->v_sh, a->v_sb))
+    return attn_fwd_wgmma_launch(a, p, s);
+  attn_fwd_kernel<<<dim3(p.nqt, p.H, p.B), 128, 0, s>>>(p);
+  DVLA_CHECK_LAUNCH("attn_fwd");
+  return DVLA_OK;
+}
+
+extern "C" int dvla_attn_bwd(const dvla_attn_bwd_args* a, void* stream) {
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (!a) { set_error("attn_bwd: null args"); return DVLA_ERR_INVALID; }
   if (!strides_ok(a->q, a->q_sb, a->q_ss, a->q_sh) || !strides_ok(a->k, a->k_sb, a->k_ss, a->k_sh) ||
       !strides_ok(a->v, a->v_sb, a->v_ss, a->v_sh) || !strides_ok(a->o, a->o_sb, a->o_ss, a->o_sh) ||
@@ -1131,36 +1130,22 @@ int attn_bwd_dispatch(const dvla_attn_bwd_args* a, cudaStream_t s) {
   if (!a->lse || !a->delta) { set_error("attn_bwd: lse/delta null"); return DVLA_ERR_INVALID; }
   if (a->B <= 0 || a->H <= 0 || a->Lq <= 0 || a->Lk <= 0) { set_error("attn_bwd: non-positive dims"); return DVLA_ERR_INVALID; }
   if (a->mask && !a->tile_flags) { set_error("attn_bwd: mask given without tile_flags"); return DVLA_ERR_INVALID; }
-  if (!(a->dropout_p >= 0.f && a->dropout_p < 1.f)) { set_error("attn_bwd: dropout_p out of range [0, 1)"); return DVLA_ERR_INVALID; }
-  AttnParams p;
-  memset(&p, 0, sizeof(p));
-  p.q = (const bf16*)a->q; p.k = (const bf16*)a->k; p.v = (const bf16*)a->v; p.o = (const bf16*)a->o; p.d_o = (const bf16*)a->d_o;
-  p.dq = (bf16*)a->dq; p.dk = (bf16*)a->dk; p.dv = (bf16*)a->dv;
-  p.lse = const_cast<float*>(a->lse); p.delta = a->delta;
-  p.mask = a->mask; p.tile_flags = a->mask ? a->tile_flags : nullptr;
-  p.B = (int)a->B; p.H = (int)a->H; p.Lq = (int)a->Lq; p.Lk = (int)a->Lk;
-  p.nqt = (p.Lq + 63) / 64; p.nkt = (p.Lk + 63) / 64; p.mask_words = a->mask_words;
-  p.q_sb = a->q_sb; p.q_ss = a->q_ss; p.q_sh = a->q_sh; p.k_sb = a->k_sb; p.k_ss = a->k_ss; p.k_sh = a->k_sh;
-  p.v_sb = a->v_sb; p.v_ss = a->v_ss; p.v_sh = a->v_sh; p.o_sb = a->o_sb; p.o_ss = a->o_ss; p.o_sh = a->o_sh;
-  p.do_sb = a->do_sb; p.do_ss = a->do_ss; p.do_sh = a->do_sh;
-  p.dq_sb = a->dq_sb; p.dq_ss = a->dq_ss; p.dq_sh = a->dq_sh; p.dk_sb = a->dk_sb; p.dk_ss = a->dk_ss; p.dk_sh = a->dk_sh;
-  p.dv_sb = a->dv_sb; p.dv_ss = a->dv_ss; p.dv_sh = a->dv_sh;
-  p.scale = a->scale;
-  if (a->dropout_p > 0.f) {
-    p.drop_thresh = (uint32_t)(a->dropout_p * 65536.0f + 0.5f);
-    p.drop_scale = 1.0f / (1.0f - (float)p.drop_thresh / 65536.0f);
-    p.drop_seed = a->dropout_seed;
-    p.drop_seed_ptr = a->dropout_seed_ptr;
-  }
+  if (!dropout_rate_ok(a->dropout_p)) { set_error("attn_bwd: dropout_p out of range [0, 1)"); return DVLA_ERR_INVALID; }
   if (a->key_bias) {
     if (!attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p)) {
       set_error("attn_bwd: key_bias needs the short-sequence kernels (Lq <= 32, Lk <= 64, no mask, no dropout)");
       return DVLA_ERR_UNSUPPORTED;
     }
-    return attn_small_bwd_dispatch(a, s);
+    return attn_small_bwd(a, s);
   }
   if (attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p))
-    return attn_small_bwd_dispatch(a, s);          // writes delta itself
+    return attn_small_bwd(a, s);          // writes delta itself
+  AttnParams p = attn_params(a);
+  p.o = (const bf16*)a->o; p.d_o = (const bf16*)a->d_o; p.dq = (bf16*)a->dq; p.dk = (bf16*)a->dk; p.dv = (bf16*)a->dv;
+  p.delta = a->delta;
+  p.do_sb = a->do_sb; p.do_ss = a->do_ss; p.do_sh = a->do_sh;
+  p.dq_sb = a->dq_sb; p.dq_ss = a->dq_ss; p.dq_sh = a->dq_sh; p.dk_sb = a->dk_sb; p.dk_ss = a->dk_ss; p.dk_sh = a->dk_sh;
+  p.dv_sb = a->dv_sb; p.dv_ss = a->dv_ss; p.dv_sh = a->dv_sh;
   const long long rows = (long long)p.B * p.H * p.Lq;
   attn_delta_kernel<<<(unsigned)((rows * 8 + 255) / 256), 256, 0, s>>>(p);
   DVLA_CHECK_LAUNCH("attn_delta");
@@ -1188,8 +1173,9 @@ int attn_bwd_dispatch(const dvla_attn_bwd_args* a, cudaStream_t s) {
   return DVLA_OK;
 }
 
-int attn_mask_tiles_dispatch(const uint32_t* mask, int32_t mask_words, int64_t Lq, int64_t Lk, uint8_t* flags,
-                             cudaStream_t s) {
+extern "C" int dvla_attn_mask_tiles(const uint32_t* mask, int32_t mask_words, int64_t Lq, int64_t Lk, uint8_t* flags,
+                                    void* stream) {
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (!mask || !flags) { set_error("attn_mask_tiles: null pointer"); return DVLA_ERR_INVALID; }
   if (mask_words * 32 < Lk) { set_error("attn_mask_tiles: mask_words too small"); return DVLA_ERR_INVALID; }
   const int nqt = (int)((Lq + 63) / 64), nkt = (int)((Lk + 63) / 64);
@@ -1199,4 +1185,6 @@ int attn_mask_tiles_dispatch(const uint32_t* mask, int32_t mask_words, int64_t L
   return DVLA_OK;
 }
 
-}  // namespace dvla
+extern "C" int64_t dvla_attn_bwd_workspace_bytes(int64_t B, int64_t H, int64_t Lq) {
+  return (B > 0 && H > 0 && Lq > 0) ? 4 * B * H * Lq : 0;
+}

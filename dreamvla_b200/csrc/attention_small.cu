@@ -10,12 +10,10 @@
 //   backward:  dQ: thread pair = one query row (also writes delta = rowsum(dO * O)); dK/dV: thread pair = one KEY row,
 //              loop over the <= 32 queries with the stored LSE -- no atomics.
 #include "common.cuh"
+#include "host.cuh"
 #include "../../include/dvla.h"
 
 namespace dvla {
-void set_error(const char* fmt, ...);
-void count_launch();
-
 namespace {
 
 constexpr float SM_LOG2E = 1.4426950408889634f;
@@ -171,12 +169,16 @@ __global__ void __launch_bounds__(256) attn_small_bwd_dkv_kernel(const SmallPara
   }
 }
 
-#define DVLA_SMALL_CHECK(name)                                                                                  \
-  do {                                                                                                          \
-    cudaError_t e__ = cudaGetLastError();                                                                       \
-    if (e__ != cudaSuccess) { set_error("%s launch: %s", name, cudaGetErrorString(e__)); return DVLA_ERR_CUDA; } \
-    count_launch();                                                                                             \
-  } while (0)
+// The SmallParams fields the forward and backward share: operands q/k/v and lse, dims, strides, scale and key bias.
+template <class Args>
+SmallParams small_params(const Args* a) {
+  SmallParams p{};
+  p.q = (const bf16*)a->q; p.k = (const bf16*)a->k; p.v = (const bf16*)a->v; p.lse = const_cast<float*>(a->lse);
+  p.B = (int)a->B; p.H = (int)a->H; p.Lq = (int)a->Lq; p.Lk = (int)a->Lk; p.scale = a->scale; p.key_bias = a->key_bias;
+  p.q_sb = a->q_sb; p.q_ss = a->q_ss; p.q_sh = a->q_sh; p.k_sb = a->k_sb; p.k_ss = a->k_ss; p.k_sh = a->k_sh;
+  p.v_sb = a->v_sb; p.v_ss = a->v_ss; p.v_sh = a->v_sh; p.o_sb = a->o_sb; p.o_ss = a->o_ss; p.o_sh = a->o_sh;
+  return p;
+}
 
 }  // namespace
 
@@ -189,33 +191,27 @@ bool attn_small_applicable(int64_t Lq, int64_t Lk, const void* mask, float dropo
   return Lq <= SMALL_MAX_LQ && Lk <= SMALL_MAX_LK && !mask && dropout_p == 0.f;
 }
 
-int attn_small_fwd_dispatch(const dvla_attn_fwd_args* a, cudaStream_t s) {
-  SmallParams p{};
-  p.q = (const bf16*)a->q; p.k = (const bf16*)a->k; p.v = (const bf16*)a->v; p.out = (bf16*)a->o; p.lse = a->lse;
-  p.B = (int)a->B; p.H = (int)a->H; p.Lq = (int)a->Lq; p.Lk = (int)a->Lk; p.scale = a->scale; p.key_bias = a->key_bias;
-  p.q_sb = a->q_sb; p.q_ss = a->q_ss; p.q_sh = a->q_sh; p.k_sb = a->k_sb; p.k_ss = a->k_ss; p.k_sh = a->k_sh;
-  p.v_sb = a->v_sb; p.v_ss = a->v_ss; p.v_sh = a->v_sh; p.o_sb = a->o_sb; p.o_ss = a->o_ss; p.o_sh = a->o_sh;
+int attn_small_fwd(const dvla_attn_fwd_args* a, cudaStream_t s) {
+  SmallParams p = small_params(a);
+  p.out = (bf16*)a->o;
   const long long threads = 2ll * a->B * a->H * a->Lq;
   attn_small_fwd_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(p);
-  DVLA_SMALL_CHECK("attn_small_fwd");
+  DVLA_CHECK_LAUNCH("attn_small_fwd");
   return DVLA_OK;
 }
 
-int attn_small_bwd_dispatch(const dvla_attn_bwd_args* a, cudaStream_t s) {
-  SmallParams p{};
-  p.q = (const bf16*)a->q; p.k = (const bf16*)a->k; p.v = (const bf16*)a->v; p.o = (const bf16*)a->o; p.d_o = (const bf16*)a->d_o;
-  p.dq = (bf16*)a->dq; p.dk = (bf16*)a->dk; p.dv = (bf16*)a->dv; p.lse = const_cast<float*>(a->lse); p.delta = a->delta;
-  p.B = (int)a->B; p.H = (int)a->H; p.Lq = (int)a->Lq; p.Lk = (int)a->Lk; p.scale = a->scale; p.key_bias = a->key_bias;
-  p.q_sb = a->q_sb; p.q_ss = a->q_ss; p.q_sh = a->q_sh; p.k_sb = a->k_sb; p.k_ss = a->k_ss; p.k_sh = a->k_sh;
-  p.v_sb = a->v_sb; p.v_ss = a->v_ss; p.v_sh = a->v_sh; p.o_sb = a->o_sb; p.o_ss = a->o_ss; p.o_sh = a->o_sh;
+int attn_small_bwd(const dvla_attn_bwd_args* a, cudaStream_t s) {
+  SmallParams p = small_params(a);
+  p.o = (const bf16*)a->o; p.d_o = (const bf16*)a->d_o; p.dq = (bf16*)a->dq; p.dk = (bf16*)a->dk; p.dv = (bf16*)a->dv;
+  p.delta = a->delta;
   p.do_sb = a->do_sb; p.do_ss = a->do_ss; p.do_sh = a->do_sh;
   p.dq_sb = a->dq_sb; p.dq_ss = a->dq_ss; p.dq_sh = a->dq_sh; p.dk_sb = a->dk_sb; p.dk_ss = a->dk_ss; p.dk_sh = a->dk_sh;
   p.dv_sb = a->dv_sb; p.dv_ss = a->dv_ss; p.dv_sh = a->dv_sh;
   const long long tq = 2ll * a->B * a->H * a->Lq, tk = 2ll * a->B * a->H * a->Lk;
   attn_small_bwd_dq_kernel<<<(unsigned)((tq + 255) / 256), 256, 0, s>>>(p);
-  DVLA_SMALL_CHECK("attn_small_bwd_dq");
+  DVLA_CHECK_LAUNCH("attn_small_bwd_dq");
   attn_small_bwd_dkv_kernel<<<(unsigned)((tk + 255) / 256), 256, 0, s>>>(p);
-  DVLA_SMALL_CHECK("attn_small_bwd_dkv");
+  DVLA_CHECK_LAUNCH("attn_small_bwd_dkv");
   return DVLA_OK;
 }
 

@@ -16,24 +16,15 @@
 // frames, the reference's `image_processor` (collator :175-179, :1311-1312; rollouts eval_utils_calvin.py:82-90,
 // eval_utils_libero.py:94-106).  Pillow resizes 8-bit images in two separable integer passes (horizontal, then vertical) with
 // 22-bit fixed-point coefficients and rounds to uint8 between them, so the crop is reproduced bit for bit: the coefficients are
-// Pillow's own computation (bicubic_coeffs below, host double arithmetic), the passes its integer sums.  Normalize is a
+// Pillow's own computation (dvla_bicubic_coeffs below, host double arithmetic), the passes its integer sums.  Normalize is a
 // [3, 256] table the caller fills with torch's own arithmetic.
 #include <math.h>
 
 #include "common.cuh"
+#include "host.cuh"
 #include "../../include/dvla.h"
 
 namespace dvla {
-void set_error(const char* fmt, ...);
-void count_launch();
-int num_sms();
-
-#define DVLA_CHECK_LAUNCH(name)                                                                 \
-  do {                                                                                          \
-    cudaError_t e__ = cudaGetLastError();                                                       \
-    if (e__ != cudaSuccess) { set_error("%s launch: %s", name, cudaGetErrorString(e__)); return DVLA_ERR_CUDA; } \
-    count_launch();                                                                             \
-  } while (0)
 
 template <typename T> __device__ __forceinline__ float ld_as_float(const T* p);
 template <> __device__ __forceinline__ float ld_as_float<float>(const float* p) { return __ldg(p); }
@@ -83,43 +74,6 @@ static unsigned grid_for(long long total) {
   return static_cast<unsigned>(blocks < cap ? (blocks > 0 ? blocks : 1) : cap);
 }
 
-// dtype codes: 0 = fp32, 1 = bf16
-int shift_crop_dispatch(const void* x, void* out, const int32_t* shifts, int64_t n, int64_t c, int64_t h, int64_t w, int32_t pad,
-                        int32_t in_dtype, int32_t out_dtype, cudaStream_t s) {
-  if (n == 0) return DVLA_OK;
-  if (!x || !out || !shifts) { set_error("shift_crop: null pointer"); return DVLA_ERR_INVALID; }
-  if (n < 0 || c <= 0 || h <= 0 || w <= 0 || pad < 0 || h > 32768 || w > 32768 || c > 65535) { set_error("shift_crop: bad dims"); return DVLA_ERR_INVALID; }
-  if ((in_dtype | out_dtype) & ~1) { set_error("shift_crop: dtype codes are 0 (fp32) / 1 (bf16)"); return DVLA_ERR_INVALID; }
-  const unsigned g = grid_for(n * c * h * 32);          // one warp per row
-#define SC(TI, TO) shift_crop_kernel<TI, TO><<<g, 256, 0, s>>>((const TI*)x, (TO*)out, shifts, n, (int)c, (int)h, (int)w, pad)
-  switch (in_dtype * 2 + out_dtype) {
-    case 0: SC(float, float); break;
-    case 1: SC(float, bf16); break;
-    case 2: SC(bf16, float); break;
-    default: SC(bf16, bf16); break;
-  }
-#undef SC
-  DVLA_CHECK_LAUNCH("shift_crop");
-  return DVLA_OK;
-}
-
-int resize_nearest_dispatch(const float* x, void* out, int64_t n, int64_t hin, int64_t win, int64_t hout, int64_t wout,
-                            int32_t out_dtype, cudaStream_t s) {
-  if (n == 0) return DVLA_OK;
-  if (!x || !out) { set_error("resize_nearest: null pointer"); return DVLA_ERR_INVALID; }
-  if (n < 0 || hin <= 0 || win <= 0 || hout <= 0 || wout <= 0 || hin > 32768 || win > 32768 || hout > 32768 || wout > 32768) {
-    set_error("resize_nearest: bad dims"); return DVLA_ERR_INVALID;
-  }
-  if (out_dtype & ~1) { set_error("resize_nearest: dtype codes are 0 (fp32) / 1 (bf16)"); return DVLA_ERR_INVALID; }
-  if (n == 0) return DVLA_OK;
-  const float sh = static_cast<float>(hin) / static_cast<float>(hout), sw = static_cast<float>(win) / static_cast<float>(wout);
-  const unsigned g = grid_for(n * hout * wout);
-  if (out_dtype == 0) resize_nearest_kernel<float><<<g, 256, 0, s>>>(x, (float*)out, n, (int)hin, (int)win, (int)hout, (int)wout, sh, sw);
-  else                resize_nearest_kernel<bf16><<<g, 256, 0, s>>>(x, (bf16*)out, n, (int)hin, (int)win, (int)hout, (int)wout, sh, sw);
-  DVLA_CHECK_LAUNCH("resize_nearest");
-  return DVLA_OK;
-}
-
 // ---- image_fn ----------------------------------------------------------------------------------------------------------------
 constexpr int kCrop = 224;                 // CLIP ViT input side
 constexpr int kPrecisionBits = 22;         // Pillow Resample.c PRECISION_BITS = 32 - 8 - 2
@@ -166,45 +120,6 @@ static void image_fn_geometry(int64_t h, int64_t w, int64_t* rh, int64_t* rw, in
   auto offset = [](int64_t d) { const int64_t k = d / 2; return (d % 2 == 0 || k % 2 == 0) ? k : k + 1; };
   *top = offset(*rh - kCrop);
   *left = offset(*rw - kCrop);
-}
-
-int bicubic_taps(int64_t in_size, int64_t out_size) {
-  if (in_size <= 0 || out_size <= 0 || in_size > (1 << 20) || out_size > (1 << 20)) {
-    set_error("bicubic_taps: sizes must be in [1, 2^20]"); return DVLA_ERR_INVALID;
-  }
-  return in_size == out_size ? 1 : BicubicLine(in_size, out_size).taps;
-}
-
-int bicubic_coeffs(int64_t in_size, int64_t out_size, int64_t first, int64_t count, int32_t* bounds, int32_t* coeffs) {
-  const int taps = bicubic_taps(in_size, out_size);
-  if (taps < 0) return taps;
-  if (!bounds || !coeffs) { set_error("bicubic_coeffs: null pointer"); return DVLA_ERR_INVALID; }
-  if (first < 0 || count < 0 || first + count > out_size) { set_error("bicubic_coeffs: outputs out of range"); return DVLA_ERR_INVALID; }
-  const BicubicLine line(in_size, out_size);
-  const double ss = 1.0 / line.filterscale;
-  for (int64_t i = 0; i < count; ++i) {
-    int32_t* c = coeffs + i * taps;
-    for (int t = 0; t < taps; ++t) c[t] = 0;
-    if (in_size == out_size) {                             // Pillow skips the pass: the identity
-      bounds[2 * i] = static_cast<int32_t>(first + i);
-      bounds[2 * i + 1] = 1;
-      c[0] = 1 << kPrecisionBits;
-      continue;
-    }
-    int xmin, n;
-    double center;
-    line.bounds(in_size, first + i, &xmin, &n, &center);
-    double ww = 0.0;
-    for (int x = 0; x < n; ++x) ww += bicubic_filter((x + xmin - center + 0.5) * ss);
-    for (int x = 0; x < n; ++x) {
-      const double f = bicubic_filter((x + xmin - center + 0.5) * ss);     // the same value again: no scratch buffer
-      const double v = ww != 0.0 ? f / ww : f;
-      c[x] = static_cast<int32_t>(v < 0 ? -0.5 + v * (1 << kPrecisionBits) : 0.5 + v * (1 << kPrecisionBits));
-    }
-    bounds[2 * i] = xmin;
-    bounds[2 * i + 1] = n;
-  }
-  return DVLA_OK;
 }
 
 __device__ __forceinline__ uint8_t clip8(int v) {          // Pillow clip8: >> 22 with saturation
@@ -291,7 +206,91 @@ __global__ void __launch_bounds__(256) image_fn_kernel(const uint8_t* __restrict
   }
 }
 
-int image_fn_dispatch(const dvla_image_fn_args* a, cudaStream_t s) {
+}  // namespace dvla
+
+using namespace dvla;
+
+// dtype codes: 0 = fp32, 1 = bf16
+extern "C" int dvla_shift_crop(const void* x, void* out, const int32_t* shifts, int64_t n, int64_t c, int64_t h, int64_t w,
+                               int32_t pad, int32_t in_dtype, int32_t out_dtype, void* stream) {
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  if (n == 0) return DVLA_OK;
+  if (!x || !out || !shifts) { set_error("shift_crop: null pointer"); return DVLA_ERR_INVALID; }
+  if (n < 0 || c <= 0 || h <= 0 || w <= 0 || pad < 0 || h > 32768 || w > 32768 || c > 65535) { set_error("shift_crop: bad dims"); return DVLA_ERR_INVALID; }
+  if ((in_dtype | out_dtype) & ~1) { set_error("shift_crop: dtype codes are 0 (fp32) / 1 (bf16)"); return DVLA_ERR_INVALID; }
+  const unsigned g = grid_for(n * c * h * 32);          // one warp per row
+#define SC(TI, TO) shift_crop_kernel<TI, TO><<<g, 256, 0, s>>>((const TI*)x, (TO*)out, shifts, n, (int)c, (int)h, (int)w, pad)
+  switch (in_dtype * 2 + out_dtype) {
+    case 0: SC(float, float); break;
+    case 1: SC(float, bf16); break;
+    case 2: SC(bf16, float); break;
+    default: SC(bf16, bf16); break;
+  }
+#undef SC
+  DVLA_CHECK_LAUNCH("shift_crop");
+  return DVLA_OK;
+}
+
+extern "C" int dvla_resize_nearest(const float* x, void* out, int64_t n, int64_t hin, int64_t win, int64_t hout, int64_t wout,
+                                   int32_t out_dtype, void* stream) {
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  if (n == 0) return DVLA_OK;
+  if (!x || !out) { set_error("resize_nearest: null pointer"); return DVLA_ERR_INVALID; }
+  if (n < 0 || hin <= 0 || win <= 0 || hout <= 0 || wout <= 0 || hin > 32768 || win > 32768 || hout > 32768 || wout > 32768) {
+    set_error("resize_nearest: bad dims"); return DVLA_ERR_INVALID;
+  }
+  if (out_dtype & ~1) { set_error("resize_nearest: dtype codes are 0 (fp32) / 1 (bf16)"); return DVLA_ERR_INVALID; }
+  if (n == 0) return DVLA_OK;
+  const float sh = static_cast<float>(hin) / static_cast<float>(hout), sw = static_cast<float>(win) / static_cast<float>(wout);
+  const unsigned g = grid_for(n * hout * wout);
+  if (out_dtype == 0) resize_nearest_kernel<float><<<g, 256, 0, s>>>(x, (float*)out, n, (int)hin, (int)win, (int)hout, (int)wout, sh, sw);
+  else                resize_nearest_kernel<bf16><<<g, 256, 0, s>>>(x, (bf16*)out, n, (int)hin, (int)win, (int)hout, (int)wout, sh, sw);
+  DVLA_CHECK_LAUNCH("resize_nearest");
+  return DVLA_OK;
+}
+
+extern "C" int32_t dvla_bicubic_taps(int64_t in_size, int64_t out_size) {
+  if (in_size <= 0 || out_size <= 0 || in_size > (1 << 20) || out_size > (1 << 20)) {
+    set_error("bicubic_taps: sizes must be in [1, 2^20]"); return DVLA_ERR_INVALID;
+  }
+  return in_size == out_size ? 1 : BicubicLine(in_size, out_size).taps;
+}
+
+extern "C" int dvla_bicubic_coeffs(int64_t in_size, int64_t out_size, int64_t first, int64_t count, int32_t* bounds,
+                                   int32_t* coeffs) {
+  const int taps = dvla_bicubic_taps(in_size, out_size);
+  if (taps < 0) return taps;
+  if (!bounds || !coeffs) { set_error("bicubic_coeffs: null pointer"); return DVLA_ERR_INVALID; }
+  if (first < 0 || count < 0 || first + count > out_size) { set_error("bicubic_coeffs: outputs out of range"); return DVLA_ERR_INVALID; }
+  const BicubicLine line(in_size, out_size);
+  const double ss = 1.0 / line.filterscale;
+  for (int64_t i = 0; i < count; ++i) {
+    int32_t* c = coeffs + i * taps;
+    for (int t = 0; t < taps; ++t) c[t] = 0;
+    if (in_size == out_size) {                             // Pillow skips the pass: the identity
+      bounds[2 * i] = static_cast<int32_t>(first + i);
+      bounds[2 * i + 1] = 1;
+      c[0] = 1 << kPrecisionBits;
+      continue;
+    }
+    int xmin, n;
+    double center;
+    line.bounds(in_size, first + i, &xmin, &n, &center);
+    double ww = 0.0;
+    for (int x = 0; x < n; ++x) ww += bicubic_filter((x + xmin - center + 0.5) * ss);
+    for (int x = 0; x < n; ++x) {
+      const double f = bicubic_filter((x + xmin - center + 0.5) * ss);     // the same value again: no scratch buffer
+      const double v = ww != 0.0 ? f / ww : f;
+      c[x] = static_cast<int32_t>(v < 0 ? -0.5 + v * (1 << kPrecisionBits) : 0.5 + v * (1 << kPrecisionBits));
+    }
+    bounds[2 * i] = xmin;
+    bounds[2 * i + 1] = n;
+  }
+  return DVLA_OK;
+}
+
+extern "C" int dvla_image_fn(const dvla_image_fn_args* a, void* stream) {
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (!a) { set_error("image_fn: null args"); return DVLA_ERR_INVALID; }
   if (a->n == 0) return DVLA_OK;
   if (!a->frames || !a->out || !a->xbounds || !a->xcoeffs || !a->ybounds || !a->ycoeffs || !a->lut) {
@@ -307,7 +306,7 @@ int image_fn_dispatch(const dvla_image_fn_args* a, cudaStream_t s) {
   if ((reinterpret_cast<uintptr_t>(a->out) & 15) != 0) { set_error("image_fn: out must be 16-byte aligned"); return DVLA_ERR_INVALID; }
   int64_t rh, rw, top, left;
   image_fn_geometry(a->h, a->w, &rh, &rw, &top, &left);
-  const int kx = bicubic_taps(a->w, rw), ky = bicubic_taps(a->h, rh);
+  const int kx = dvla_bicubic_taps(a->w, rw), ky = dvla_bicubic_taps(a->h, rh);
   // the largest band of output rows whose staged input rows fit the shared-memory budget (bounds as dvla_bicubic_coeffs gives them)
   const BicubicLine line(a->h, rh);
   auto row_bound = [&](int y, bool end) {                    // first input row output row y reads, or (end) one past its last
@@ -333,5 +332,3 @@ int image_fn_dispatch(const dvla_image_fn_args* a, cudaStream_t s) {
   DVLA_CHECK_LAUNCH("image_fn");
   return DVLA_OK;
 }
-
-}  // namespace dvla

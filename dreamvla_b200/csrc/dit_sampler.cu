@@ -20,15 +20,12 @@
 #include <string.h>
 
 #include "common.cuh"
+#include "host.cuh"
 #include "../../include/dvla.h"
 
 namespace cg = cooperative_groups;
 
 namespace dvla {
-void set_error(const char* fmt, ...);
-void count_launch();
-int num_sms();
-
 namespace {
 
 constexpr int DS_THREADS = 512;      // 16 warps per SM: the skinny GEMMs hide weight-load latency with warps in flight
@@ -406,7 +403,12 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dit_ddim_sample_kernel(const __
 
 }  // namespace
 
-int dit_ddim_sample_dispatch(const dvla_dit_sampler_args* a, cudaStream_t s) {
+}  // namespace dvla
+
+using namespace dvla;
+
+extern "C" int dvla_dit_ddim_sample(const dvla_dit_sampler_args* a, void* stream) {
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (!a || !a->blocks || !a->z || !a->noise || !a->out || !a->workspace) { set_error("dit_ddim_sample: null pointer"); return DVLA_ERR_INVALID; }
   const int H = (int)a->hidden, T = (int)a->T, C = (int)a->channels, bs = (int)a->batch;
   const int M = 2 * bs * 2 * T;
@@ -471,8 +473,6 @@ int dit_ddim_sample_dispatch(const dvla_dit_sampler_args* a, cudaStream_t s) {
   count_launch();
   return DVLA_OK;
 }
-
-}  // namespace dvla
 
 extern "C" int64_t dvla_dit_sampler_workspace_bytes(int64_t batch, int64_t T, int64_t hidden, int64_t mlp, int64_t n_steps) {
   const int64_t M = 2 * batch * 2 * T;

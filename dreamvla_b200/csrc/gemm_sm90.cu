@@ -14,6 +14,7 @@
 //
 // Replaces the cuBLAS calls behind nn.Linear / Conv1D in the reference (see include/dvla.h for call sites).
 #include "common.cuh"
+#include "host.cuh"
 #include "../../include/dvla.h"
 
 namespace dvla {
@@ -610,9 +611,6 @@ __global__ void gemm_simt_warp_kernel(const bf16* __restrict__ a, const bf16* __
 #include <string.h>
 
 namespace dvla {
-void set_error(const char* fmt, ...);
-void count_launch();
-int num_sms();
 
 // dvla_gemm_plan: the dispatcher runs as usual up to the point where it would encode tensor maps and launch; with this
 // thread-local set it records its decisions instead (host only -- no CUDA call, usable without a GPU)
@@ -627,10 +625,7 @@ static void record_plan(const GemmParams& p, int kernel, int tile_m, int tile_n,
   o.grid_ctas = grid_ctas;
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn get_encode_fn() {
+EncodeTiledFn get_encode_fn() {
   static EncodeTiledFn fn = nullptr;
   static std::once_flag once;
   std::call_once(once, [] {
@@ -642,8 +637,6 @@ static EncodeTiledFn get_encode_fn() {
   });
   return fn;
 }
-
-EncodeTiledFn get_encode_fn_shared() { return get_encode_fn(); }
 
 // Descriptor cache (SURVEY 8b): the only mutable module-level state besides the launch counter.  Keyed by everything
 // cuTensorMapEncodeTiled sees; guarded by a mutex because forward (main thread) and backward (autograd's device thread)
@@ -727,9 +720,7 @@ static int launch_tc(const dvla_gemm_args* a, const GemmParams& p, cudaStream_t 
     set_error("cudaFuncSetAttribute(smem=%d): %s", Cfg::SMEM_BYTES, cudaGetErrorString(attr_err)); return DVLA_ERR_CUDA;
   }
   kern<<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, p);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { set_error("gemm_wgmma launch: %s", cudaGetErrorString(e)); return DVLA_ERR_CUDA; }
-  count_launch();
+  DVLA_CHECK_LAUNCH("gemm_wgmma");
   return DVLA_OK;
 }
 
@@ -754,7 +745,6 @@ static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t
 constexpr int64_t TAIL_CNT_BYTES = 65536;
 constexpr int64_t TAIL_WS_SLICES = 132;              // 128 x 128 fp32 slices (8.25 MB): a split tail wave needs <= 132 (one
                                                      // per SM)
-int64_t gemm_workspace_bytes() { return TAIL_CNT_BYTES + TAIL_WS_SLICES * BM * BN * 4; }
 
 static bool tail_fits(const dvla_gemm_args* a, long long tail_tiles, int splits) {
   if (!a->workspace || (reinterpret_cast<uintptr_t>(a->workspace) & 15)) return false;
@@ -789,11 +779,16 @@ static void plan_tail(GemmParams& p, const dvla_gemm_args* a, long long total_ti
   p.tail_ws = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(a->workspace) + TAIL_CNT_BYTES);
 }
 
-int gemm_dispatch(const dvla_gemm_args* a, cudaStream_t stream) {
+}  // namespace dvla
+
+using namespace dvla;
+
+extern "C" int dvla_gemm(const dvla_gemm_args* a, void* stream) {
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (!a || !a->a || !a->b || !a->out) { set_error("dvla_gemm: null pointer"); return DVLA_ERR_INVALID; }
   if (a->M <= 0 || a->N <= 0 || a->K <= 0) { set_error("dvla_gemm: non-positive dims M=%lld N=%lld K=%lld", (long long)a->M, (long long)a->N, (long long)a->K); return DVLA_ERR_INVALID; }
   if (a->aux_in && a->aux_out) { set_error("dvla_gemm: aux_in and aux_out are exclusive"); return DVLA_ERR_INVALID; }
-  if (!(a->dropout_p >= 0.f && a->dropout_p < 1.f)) { set_error("dvla_gemm: dropout_p out of range"); return DVLA_ERR_INVALID; }
+  if (!dropout_rate_ok(a->dropout_p)) { set_error("dvla_gemm: dropout_p out of range"); return DVLA_ERR_INVALID; }
   GemmParams p;
   memset(&p, 0, sizeof(p));
   p.out = a->out; p.bias = (const bf16*)a->bias; p.residual = a->residual;
@@ -802,8 +797,7 @@ int gemm_dispatch(const dvla_gemm_args* a, cudaStream_t stream) {
   p.ldo = a->ldo; p.ldr = a->ldr; p.ld_aux = a->ld_aux;
   p.act = a->act; p.out_fp32 = a->out_fp32; p.alpha = a->alpha;
   if (a->dropout_p > 0.f) {
-    p.drop_thresh = (uint32_t)(a->dropout_p * 65536.0f + 0.5f);
-    p.drop_scale = 1.0f / (1.0f - (float)p.drop_thresh / 65536.0f);
+    dropout_thresh_scale(a->dropout_p, &p.drop_thresh, &p.drop_scale);
     p.drop_seed = a->dropout_seed;
     p.drop_seed_ptr = a->dropout_seed_ptr;
   }
@@ -829,16 +823,14 @@ int gemm_dispatch(const dvla_gemm_args* a, cudaStream_t stream) {
     }
     if (p.K >= 128 && groups <= 65536) {      // long contraction, small output: one warp per output group
       const long long blocks = (groups * 32 + threads - 1) / threads;
-      gemm_simt_warp_kernel<<<(unsigned)blocks, threads, 0, stream>>>((const bf16*)a->a, (const bf16*)a->b, a->lda, a->ldb,
-                                                                    a->a_mn_major, a->b_mn_major, p);
+      gemm_simt_warp_kernel<<<(unsigned)blocks, threads, 0, s>>>((const bf16*)a->a, (const bf16*)a->b, a->lda, a->ldb,
+                                                               a->a_mn_major, a->b_mn_major, p);
     } else {
       const long long blocks = (groups + threads - 1) / threads;
-      gemm_simt_kernel<<<(unsigned)blocks, threads, 0, stream>>>((const bf16*)a->a, (const bf16*)a->b, a->lda, a->ldb,
-                                                               a->a_mn_major, a->b_mn_major, p);
+      gemm_simt_kernel<<<(unsigned)blocks, threads, 0, s>>>((const bf16*)a->a, (const bf16*)a->b, a->lda, a->ldb,
+                                                          a->a_mn_major, a->b_mn_major, p);
     }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { set_error("gemm_simt launch: %s", cudaGetErrorString(e)); return DVLA_ERR_CUDA; }
-    count_launch();
+    DVLA_CHECK_LAUNCH("gemm_simt");
     return DVLA_OK;
   }
   const int sms = num_sms();
@@ -867,22 +859,23 @@ int gemm_dispatch(const dvla_gemm_args* a, cudaStream_t stream) {
       p.kb_per_split = (p.num_k_blocks + best_s - 1) / best_s;
       p.atomic_out = 1;
       p.residual = nullptr;
-      return launch_tc_any(a, p, stream);
+      return launch_tc_any(a, p, s);
     }
   }
   plan_tail(p, a, tiles, sms);
-  return launch_tc_any(a, p, stream);
+  return launch_tc_any(a, p, s);
 }
 
-int gemm_plan(const dvla_gemm_args* a, dvla_gemm_plan_info* out) {
+extern "C" int dvla_gemm_plan(const dvla_gemm_args* a, dvla_gemm_plan_info* out) {
   if (!out) { set_error("dvla_gemm_plan: null output"); return DVLA_ERR_INVALID; }
   memset(out, 0, sizeof(*out));
   g_plan = out;
-  const int rc = gemm_dispatch(a, nullptr);
+  const int rc = dvla_gemm(a, nullptr);
   g_plan = nullptr;
   return rc;
 }
-int gemm_plan_unit(const dvla_gemm_plan_info* plan, int unit, int* tile, int* kb0, int* kb1, int* slot, int* split) {
+extern "C" int dvla_gemm_plan_unit(const dvla_gemm_plan_info* plan, int32_t unit, int32_t* tile, int32_t* kb0, int32_t* kb1,
+                                   int32_t* slot, int32_t* split) {
   if (!plan || plan->kernel < 2 || unit < 0 || unit >= plan->units) { set_error("dvla_gemm_plan_unit: bad plan / unit"); return DVLA_ERR_INVALID; }
   GemmParams p;
   memset(&p, 0, sizeof(p));
@@ -897,4 +890,4 @@ int gemm_plan_unit(const dvla_gemm_plan_info* plan, int unit, int* tile, int* kb
   return DVLA_OK;
 }
 
-}  // namespace dvla
+extern "C" int64_t dvla_gemm_workspace_bytes(const dvla_gemm_args*) { return TAIL_CNT_BYTES + TAIL_WS_SLICES * BM * BN * 4; }

@@ -1,19 +1,10 @@
 // Fused loss kernels (value + gradient in one pass) and the flat-buffer optimiser (grad-norm, clip, AdamW).
 // All HBM-bound: 16-byte vector accesses, grid-stride loops sized against the SM count, block reduce -> one atomicAdd.
 #include "common.cuh"
+#include "host.cuh"
 #include "../../include/dvla.h"
 
 namespace dvla {
-void set_error(const char* fmt, ...);
-void count_launch();
-int num_sms();
-
-#define DVLA_CHECK_LAUNCH(name)                                                                 \
-  do {                                                                                          \
-    cudaError_t e__ = cudaGetLastError();                                                       \
-    if (e__ != cudaSuccess) { set_error("%s launch: %s", name, cudaGetErrorString(e__)); return DVLA_ERR_CUDA; } \
-    count_launch();                                                                             \
-  } while (0)
 
 __device__ __forceinline__ float block_sum_256(float v) {
   __shared__ float red[8];
@@ -54,15 +45,6 @@ __global__ void __launch_bounds__(256) mse_loss_kernel(const bf16* __restrict__ 
   const float t = block_sum_256(acc);
   if (threadIdx.x == 0) atomicAdd(loss_out, weight * t * inv);
 }
-int mse_loss_dispatch(const void* pred, const void* label, const float* row_mask, int64_t rows, int64_t C, float weight,
-                      float* loss_out, void* dpred, cudaStream_t s) {
-  if (!pred || !label || !loss_out) { set_error("mse_loss: null pointer"); return DVLA_ERR_INVALID; }
-  if (rows <= 0 || C <= 0) return DVLA_OK;
-  mse_loss_kernel<<<grid_for(rows * C, 256 * 8), 256, 0, s>>>((const bf16*)pred, (const bf16*)label, row_mask, rows,
-                                                             (int)C, weight, loss_out, (bf16*)dpred);
-  DVLA_CHECK_LAUNCH("mse_loss");
-  return DVLA_OK;
-}
 
 // ---------------------------------------------------------------------------------------------------------------
 // mean_rows(1 - cos(pred_row, label_row))   (train_utils.py:423-425, 448-450; F.cosine_similarity eps = 1e-8)
@@ -98,15 +80,6 @@ __global__ void __launch_bounds__(256) cosine_loss_kernel(const bf16* __restrict
   const float t = block_sum_256(acc);
   if (threadIdx.x == 0) atomicAdd(loss_out, weight * t * invr);
 }
-int cosine_loss_dispatch(const void* pred, const void* label, int64_t rows, int64_t C, float weight, float* loss_out,
-                         void* dpred, cudaStream_t s) {
-  if (!pred || !label || !loss_out) { set_error("cosine_loss: null pointer"); return DVLA_ERR_INVALID; }
-  if (rows <= 0 || C <= 0) return DVLA_OK;
-  cosine_loss_kernel<<<grid_for(rows, 8), 256, 0, s>>>((const bf16*)pred, (const bf16*)label, rows, (int)C, weight,
-                                                      loss_out, (bf16*)dpred);
-  DVLA_CHECK_LAUNCH("cosine_loss");
-  return DVLA_OK;
-}
 
 // ---------------------------------------------------------------------------------------------------------------
 // Scale-invariant log loss (utils/sigloss.py:11-15): d = log(t+1e-6) - log(p+1e-6); sqrt(mean(d^2) - lambd*mean(d)^2)
@@ -140,22 +113,6 @@ __global__ void __launch_bounds__(256) silog_finish_kernel(const bf16* __restric
     // dL/dd_i = (2 d_i - 2 lambd md)/n / (2L);  dd_i/dp_i = -1/(p_i+1e-6)
     dpred[i] = __float2bfloat16(-k * (2.0f * d - 2.0f * lambd * md) * invn / pv);
   }
-}
-int silog_stats_dispatch(const void* pred, const void* label, int64_t n, float* stats, cudaStream_t s) {
-  if (!pred || !label || !stats) { set_error("silog_stats: null pointer"); return DVLA_ERR_INVALID; }
-  if (n <= 0) return DVLA_OK;
-  silog_stats_kernel<<<grid_for(n, 256 * 8), 256, 0, s>>>((const bf16*)pred, (const bf16*)label, n, stats);
-  DVLA_CHECK_LAUNCH("silog_stats");
-  return DVLA_OK;
-}
-int silog_finish_dispatch(const void* pred, const void* label, int64_t n, const float* stats, float lambd, float weight,
-                          float* loss_out, void* dpred, cudaStream_t s) {
-  if (!pred || !label || !stats || !loss_out) { set_error("silog_finish: null pointer"); return DVLA_ERR_INVALID; }
-  if (n <= 0) return DVLA_OK;
-  silog_finish_kernel<<<grid_for(n, 256 * 8), 256, 0, s>>>((const bf16*)pred, (const bf16*)label, n, stats, lambd, weight,
-                                                          loss_out, (bf16*)dpred);
-  DVLA_CHECK_LAUNCH("silog_finish");
-  return DVLA_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -202,16 +159,6 @@ __global__ void __launch_bounds__(256) sumsq_kernel(const bf16* __restrict__ g, 
     }
   }
 }
-int sumsq_dispatch(const void* g, int64_t n, float* out, cudaStream_t s) {
-  if (!g || !out) { set_error("sumsq: null pointer"); return DVLA_ERR_INVALID; }
-  if (reinterpret_cast<uintptr_t>(g) & 15) { set_error("sumsq: buffer must be 16-byte aligned"); return DVLA_ERR_INVALID; }
-  if (n <= 0) return DVLA_OK;
-  unsigned blocks = grid_for(n, 256 * 8 * 4);
-  if (blocks > SUMSQ_MAX_BLOCKS) blocks = SUMSQ_MAX_BLOCKS;
-  sumsq_kernel<<<blocks, 256, 0, s>>>((const bf16*)g, n, out);
-  DVLA_CHECK_LAUNCH("sumsq");
-  return DVLA_OK;
-}
 
 // In-place clip of the (rank-summed) accumulated gradient: g *= grad_scale * min(1, max_norm / (||g||*grad_scale + 1e-6)).
 // Reference utils/train_utils.py:599-600 clips the ACCUMULATED gradient after every micro-step; with gradient accumulation
@@ -235,14 +182,6 @@ __global__ void __launch_bounds__(256) grad_clip_scale_kernel(bf16* __restrict__
   }
   if (blockIdx.x == 0)
     for (long long i = (nv << 3) + threadIdx.x; i < n; i += blockDim.x) g[i] = __float2bfloat16(__bfloat162float(g[i]) * c);
-}
-int grad_clip_scale_dispatch(void* g, int64_t n, const float* sumsq, float max_norm, float grad_scale, cudaStream_t s) {
-  if (!g || !sumsq) { set_error("grad_clip_scale: null pointer"); return DVLA_ERR_INVALID; }
-  if (reinterpret_cast<uintptr_t>(g) & 15) { set_error("grad_clip_scale: buffer must be 16-byte aligned"); return DVLA_ERR_INVALID; }
-  if (n <= 0) return DVLA_OK;
-  grad_clip_scale_kernel<<<grid_for(n, 256 * 8 * 4), 256, 0, s>>>((bf16*)g, n, sumsq, max_norm, grad_scale);
-  DVLA_CHECK_LAUNCH("grad_clip_scale");
-  return DVLA_OK;
 }
 
 struct AdamWParams {
@@ -303,17 +242,6 @@ __global__ void __launch_bounds__(256) adamw_kernel(AdamWParams a) {
       if (a.zero_grad) a.g[i] = __float2bfloat16(0.f);
     }
   }
-}
-int adamw_dispatch(const dvla_adamw_args* a, cudaStream_t s) {
-  if (!a || !a->p || !a->g || !a->m || !a->v || !a->lr || !a->step) { set_error("adamw: null pointer"); return DVLA_ERR_INVALID; }
-  if ((reinterpret_cast<uintptr_t>(a->p) | reinterpret_cast<uintptr_t>(a->g) | reinterpret_cast<uintptr_t>(a->m) |
-       reinterpret_cast<uintptr_t>(a->v)) & 15) { set_error("adamw: buffers must be 16-byte aligned"); return DVLA_ERR_INVALID; }
-  if (a->n <= 0) return DVLA_OK;
-  AdamWParams k{(bf16*)a->p, (bf16*)a->g, a->m, a->v, a->n, a->sumsq, a->lr, a->step,
-                a->beta1, a->beta2, a->eps, a->weight_decay, a->max_norm, a->grad_scale, a->zero_grad};
-  adamw_kernel<<<grid_for(a->n, 256 * 8 * 2), 256, 0, s>>>(k);
-  DVLA_CHECK_LAUNCH("adamw");
-  return DVLA_OK;
 }
 
 // The same clip + AdamW on fp32 master weights: the update lands in p32 (no bf16 rounding of the parameter between
@@ -383,7 +311,91 @@ __global__ void __launch_bounds__(256) adamw_master_kernel(AdamWMasterParams a) 
     }
   }
 }
-int adamw_master_dispatch(const dvla_adamw_master_args* a, cudaStream_t s) {
+
+}  // namespace dvla
+
+using namespace dvla;
+
+extern "C" int dvla_mse_loss(const void* pred, const void* label, const float* row_mask, int64_t rows, int64_t C, float weight,
+                             float* loss_out, void* dpred, void* stream) {
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  if (!pred || !label || !loss_out) { set_error("mse_loss: null pointer"); return DVLA_ERR_INVALID; }
+  if (rows <= 0 || C <= 0) return DVLA_OK;
+  mse_loss_kernel<<<grid_for(rows * C, 256 * 8), 256, 0, s>>>((const bf16*)pred, (const bf16*)label, row_mask, rows,
+                                                             (int)C, weight, loss_out, (bf16*)dpred);
+  DVLA_CHECK_LAUNCH("mse_loss");
+  return DVLA_OK;
+}
+
+extern "C" int dvla_cosine_loss(const void* pred, const void* label, int64_t rows, int64_t C, float weight, float* loss_out,
+                                void* dpred, void* stream) {
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  if (!pred || !label || !loss_out) { set_error("cosine_loss: null pointer"); return DVLA_ERR_INVALID; }
+  if (rows <= 0 || C <= 0) return DVLA_OK;
+  cosine_loss_kernel<<<grid_for(rows, 8), 256, 0, s>>>((const bf16*)pred, (const bf16*)label, rows, (int)C, weight,
+                                                      loss_out, (bf16*)dpred);
+  DVLA_CHECK_LAUNCH("cosine_loss");
+  return DVLA_OK;
+}
+
+extern "C" int dvla_silog_stats(const void* pred, const void* label, int64_t n, float* stats, void* stream) {
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  if (!pred || !label || !stats) { set_error("silog_stats: null pointer"); return DVLA_ERR_INVALID; }
+  if (n <= 0) return DVLA_OK;
+  silog_stats_kernel<<<grid_for(n, 256 * 8), 256, 0, s>>>((const bf16*)pred, (const bf16*)label, n, stats);
+  DVLA_CHECK_LAUNCH("silog_stats");
+  return DVLA_OK;
+}
+
+extern "C" int dvla_silog_finish(const void* pred, const void* label, int64_t n, const float* stats, float lambd, float weight,
+                                 float* loss_out, void* dpred, void* stream) {
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  if (!pred || !label || !stats || !loss_out) { set_error("silog_finish: null pointer"); return DVLA_ERR_INVALID; }
+  if (n <= 0) return DVLA_OK;
+  silog_finish_kernel<<<grid_for(n, 256 * 8), 256, 0, s>>>((const bf16*)pred, (const bf16*)label, n, stats, lambd, weight,
+                                                          loss_out, (bf16*)dpred);
+  DVLA_CHECK_LAUNCH("silog_finish");
+  return DVLA_OK;
+}
+extern "C" int64_t dvla_silog_workspace_bytes(void) { return 2 * (int64_t)sizeof(float); }
+
+extern "C" int dvla_sumsq(const void* g, int64_t n, float* out, void* stream) {
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  if (!g || !out) { set_error("sumsq: null pointer"); return DVLA_ERR_INVALID; }
+  if (reinterpret_cast<uintptr_t>(g) & 15) { set_error("sumsq: buffer must be 16-byte aligned"); return DVLA_ERR_INVALID; }
+  if (n <= 0) return DVLA_OK;
+  unsigned blocks = grid_for(n, 256 * 8 * 4);
+  if (blocks > SUMSQ_MAX_BLOCKS) blocks = SUMSQ_MAX_BLOCKS;
+  sumsq_kernel<<<blocks, 256, 0, s>>>((const bf16*)g, n, out);
+  DVLA_CHECK_LAUNCH("sumsq");
+  return DVLA_OK;
+}
+
+extern "C" int dvla_grad_clip_scale(void* g, int64_t n, const float* sumsq, float max_norm, float grad_scale, void* stream) {
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  if (!g || !sumsq) { set_error("grad_clip_scale: null pointer"); return DVLA_ERR_INVALID; }
+  if (reinterpret_cast<uintptr_t>(g) & 15) { set_error("grad_clip_scale: buffer must be 16-byte aligned"); return DVLA_ERR_INVALID; }
+  if (n <= 0) return DVLA_OK;
+  grad_clip_scale_kernel<<<grid_for(n, 256 * 8 * 4), 256, 0, s>>>((bf16*)g, n, sumsq, max_norm, grad_scale);
+  DVLA_CHECK_LAUNCH("grad_clip_scale");
+  return DVLA_OK;
+}
+
+extern "C" int dvla_adamw(const dvla_adamw_args* a, void* stream) {
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  if (!a || !a->p || !a->g || !a->m || !a->v || !a->lr || !a->step) { set_error("adamw: null pointer"); return DVLA_ERR_INVALID; }
+  if ((reinterpret_cast<uintptr_t>(a->p) | reinterpret_cast<uintptr_t>(a->g) | reinterpret_cast<uintptr_t>(a->m) |
+       reinterpret_cast<uintptr_t>(a->v)) & 15) { set_error("adamw: buffers must be 16-byte aligned"); return DVLA_ERR_INVALID; }
+  if (a->n <= 0) return DVLA_OK;
+  AdamWParams k{(bf16*)a->p, (bf16*)a->g, a->m, a->v, a->n, a->sumsq, a->lr, a->step,
+                a->beta1, a->beta2, a->eps, a->weight_decay, a->max_norm, a->grad_scale, a->zero_grad};
+  adamw_kernel<<<grid_for(a->n, 256 * 8 * 2), 256, 0, s>>>(k);
+  DVLA_CHECK_LAUNCH("adamw");
+  return DVLA_OK;
+}
+
+extern "C" int dvla_adamw_master(const dvla_adamw_master_args* a, void* stream) {
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (!a || !a->p32 || !a->p || !a->g || !a->m || !a->v || !a->lr || !a->step) {
     set_error("adamw_master: null pointer");
     return DVLA_ERR_INVALID;
@@ -400,5 +412,3 @@ int adamw_master_dispatch(const dvla_adamw_master_args* a, cudaStream_t s) {
   DVLA_CHECK_LAUNCH("adamw_master");
   return DVLA_OK;
 }
-
-}  // namespace dvla

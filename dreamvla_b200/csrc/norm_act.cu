@@ -1,19 +1,10 @@
 // HBM-bound row kernels: LayerNorm fwd/bwd, column sums (bias grads), dropout, activation backward, fp32->bf16 folds.
 // One warp per row, 16-byte vector accesses, grids sized against the SM count.
 #include "common.cuh"
+#include "host.cuh"
 #include "../../include/dvla.h"
 
 namespace dvla {
-void set_error(const char* fmt, ...);
-void count_launch();
-int num_sms();
-
-#define DVLA_CHECK_LAUNCH(name)                                                                 \
-  do {                                                                                          \
-    cudaError_t e__ = cudaGetLastError();                                                       \
-    if (e__ != cudaSuccess) { set_error("%s launch: %s", name, cudaGetErrorString(e__)); return DVLA_ERR_CUDA; } \
-    count_launch();                                                                             \
-  } while (0)
 
 __device__ __forceinline__ void load8(const bf16* p, float (&f)[8]) {
   uint4 u = *reinterpret_cast<const uint4*>(p);
@@ -300,58 +291,6 @@ __global__ void __launch_bounds__(256, 2) layernorm_bwd_v2_kernel(const bf16* __
   }
 }
 
-int layernorm_fwd_dispatch(const dvla_layernorm_fwd_args* a, cudaStream_t stream) {
-  if (!a || !a->x || !a->y) { set_error("layernorm_fwd: null pointer"); return DVLA_ERR_INVALID; }
-  if (a->D % 8 || a->ldx % 8 || a->ldy % 8 || a->D > 1024 || a->D <= 0) {
-    set_error("layernorm_fwd: need D%%8==0, D<=1024, strides%%8==0 (D=%lld)", (long long)a->D);
-    return DVLA_ERR_UNSUPPORTED;
-  }
-  if (a->rows <= 0) return DVLA_OK;
-  const int nv = (int)((a->D + 255) / 256);
-  long long blocks = (a->rows + 7) / 8;
-  const long long cap = (long long)num_sms() * 8;
-  if (blocks > cap) blocks = cap;
-#define LN_FWD(NV) layernorm_fwd_kernel<NV><<<(unsigned)blocks, 256, 0, stream>>>((const bf16*)a->x, (const bf16*)a->gamma, \
-      (const bf16*)a->beta, (bf16*)a->y, a->mean, a->rstd, a->rows, (int)a->D, a->ldx, a->ldy, a->eps)
-  switch (nv) { case 1: LN_FWD(1); break; case 2: LN_FWD(2); break; case 3: LN_FWD(3); break; default: LN_FWD(4); break; }
-#undef LN_FWD
-  DVLA_CHECK_LAUNCH("layernorm_fwd");
-  return DVLA_OK;
-}
-
-int layernorm_bwd_dispatch(const dvla_layernorm_bwd_args* a, cudaStream_t stream) {
-  if (!a || !a->dy || !a->x || !a->mean || !a->rstd || !a->dx) { set_error("layernorm_bwd: null pointer"); return DVLA_ERR_INVALID; }
-  if (a->D % 8 || a->ld % 8 || a->D > 1024 || a->D <= 0) {
-    set_error("layernorm_bwd: need D%%8==0, D<=1024, ld%%8==0 (D=%lld)", (long long)a->D);
-    return DVLA_ERR_UNSUPPORTED;
-  }
-  if (a->rows <= 0) return DVLA_OK;
-  const int nv = (int)((a->D + 255) / 256);
-  long long blocks = (a->rows + 7) / 8;
-  if (a->D % 256 == 0 && (a->dgamma || a->dbeta) && a->rows >= 2048) {
-    const long long cap3 = 2LL * num_sms();
-    if (blocks > cap3) blocks = cap3;
-    const size_t smem = (size_t)8 * 2 * a->D * sizeof(float);
-#define LN_BWD2(NV) do { \
-      static const cudaError_t attr_e = cudaFuncSetAttribute(layernorm_bwd_v2_kernel<NV>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * 2 * NV * 256 * 4); \
-      if (attr_e != cudaSuccess) { set_error("layernorm_bwd_v2 smem attr: %s", cudaGetErrorString(attr_e)); return DVLA_ERR_CUDA; } \
-      layernorm_bwd_v2_kernel<NV><<<(unsigned)blocks, 256, smem, stream>>>((const bf16*)a->dy, (const bf16*)a->x, (const bf16*)a->gamma, \
-          a->mean, a->rstd, (bf16*)a->dx, a->dgamma, a->dbeta, a->rows, a->ld, (const bf16*)a->dres); } while (0)
-    switch (nv) { case 1: LN_BWD2(1); break; case 2: LN_BWD2(2); break; case 3: LN_BWD2(3); break; default: LN_BWD2(4); break; }
-#undef LN_BWD2
-    DVLA_CHECK_LAUNCH("layernorm_bwd_v2");
-    return DVLA_OK;
-  }
-  const long long cap = 2LL * num_sms();        // 2 resident blocks per SM; 2*D fp32 atomics per block at the end
-  if (blocks > cap) blocks = cap;
-#define LN_BWD(NV) layernorm_bwd_kernel<NV><<<(unsigned)blocks, 256, 0, stream>>>((const bf16*)a->dy, (const bf16*)a->x, \
-      (const bf16*)a->gamma, a->mean, a->rstd, (bf16*)a->dx, a->dgamma, a->dbeta, a->rows, (int)a->D, a->ld, (const bf16*)a->dres)
-  switch (nv) { case 1: LN_BWD(1); break; case 2: LN_BWD(2); break; case 3: LN_BWD(3); break; default: LN_BWD(4); break; }
-#undef LN_BWD
-  DVLA_CHECK_LAUNCH("layernorm_bwd");
-  return DVLA_OK;
-}
-
 // ------------------------------------------------------------------------------------------------------------------
 // Column sum (bias gradient): out[n] += sum_r x[r, n]
 // Block = 8 warps over a slab of 256 columns x a chunk of rows: each lane keeps 8 column partials in registers (coalesced
@@ -406,35 +345,12 @@ __global__ void __launch_bounds__(256) colsum_kernel(const bf16* __restrict__ x,
   const int col = blockIdx.x * 256 + c;
   if (col < N) atomicAdd(out + col, t);
 }
-int colsum_accum_dispatch(const void* x, int64_t rows, int64_t N, int64_t ld, float* out, cudaStream_t s) {
-  if (!x || !out) { set_error("colsum: null pointer"); return DVLA_ERR_INVALID; }
-  if (rows <= 0 || N <= 0) return DVLA_OK;
-  const int vec = (N % 8 == 0) && (ld % 8 == 0) && ((reinterpret_cast<uintptr_t>(x) & 15) == 0);
-  const int bx = (int)((N + 255) / 256);
-  int by = (int)((6LL * num_sms() + bx - 1) / bx);     // ~6 blocks of 256 threads per SM: enough loads in flight for HBM
-  if (by > (rows + 63) / 64) by = (int)((rows + 63) / 64);
-  if (by < 1) by = 1;
-  const int rpb = (int)((rows + by - 1) / by);
-  by = (int)((rows + rpb - 1) / rpb);
-  colsum_kernel<<<dim3(bx, by), 256, 0, s>>>((const bf16*)x, rows, (int)N, ld, out, rpb, vec);
-  DVLA_CHECK_LAUNCH("colsum");
-  return DVLA_OK;
-}
 
 // ------------------------------------------------------------------------------------------------------------------
 __global__ void accum_fp32_into_bf16_kernel(const float* __restrict__ src, bf16* __restrict__ dst, long long n) {
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
        i += static_cast<long long>(gridDim.x) * blockDim.x)
     dst[i] = __float2bfloat16(__bfloat162float(dst[i]) + src[i]);
-}
-int accum_fp32_into_bf16_dispatch(const float* src, void* dst, int64_t n, cudaStream_t s) {
-  if (!src || !dst) { set_error("accum_fp32_into_bf16: null pointer"); return DVLA_ERR_INVALID; }
-  if (n <= 0) return DVLA_OK;
-  long long blocks = (n + 255) / 256;
-  if (blocks > 4LL * num_sms()) blocks = 4LL * num_sms();
-  accum_fp32_into_bf16_kernel<<<(unsigned)blocks, 256, 0, s>>>(src, (bf16*)dst, n);
-  DVLA_CHECK_LAUNCH("accum_fp32_into_bf16");
-  return DVLA_OK;
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -464,22 +380,6 @@ __global__ void dropout_kernel(const bf16* __restrict__ x, bf16* __restrict__ y,
       }
     }
   }
-}
-int dropout_dispatch(const void* x, void* y, int64_t rows, int64_t N, int64_t ldx, int64_t ldy, float p, uint64_t seed,
-                     const uint64_t* seed_ptr, cudaStream_t s) {
-  if (!x || !y) { set_error("dropout: null pointer"); return DVLA_ERR_INVALID; }
-  if (!(p >= 0.f && p < 1.f)) { set_error("dropout: p out of range"); return DVLA_ERR_INVALID; }
-  if (rows <= 0 || N <= 0) return DVLA_OK;
-  const uint32_t thresh = (uint32_t)(p * 65536.0f + 0.5f);
-  const float scale = 1.0f / (1.0f - (float)thresh / 65536.0f);
-  const int vec = (N % 8 == 0) && (ldx % 8 == 0) && (ldy % 8 == 0) && ((reinterpret_cast<uintptr_t>(x) & 15) == 0) &&
-                  ((reinterpret_cast<uintptr_t>(y) & 15) == 0);
-  const long long total = rows * ((N + 7) / 8);
-  long long blocks = (total + 255) / 256;
-  if (blocks > 8LL * num_sms()) blocks = 8LL * num_sms();
-  dropout_kernel<<<(unsigned)blocks, 256, 0, s>>>((const bf16*)x, (bf16*)y, rows, (int)N, ldx, ldy, thresh, scale, seed, seed_ptr, vec);
-  DVLA_CHECK_LAUNCH("dropout");
-  return DVLA_OK;
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -511,17 +411,6 @@ __global__ void act_bwd_scalar_kernel(const bf16* __restrict__ dy, const bf16* _
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
        i += static_cast<long long>(gridDim.x) * blockDim.x)
     dx[i] = __float2bfloat16(__bfloat162float(dy[i]) * act_bwd(__bfloat162float(pre[i]), act));
-}
-int act_bwd_dispatch(const void* dy, const void* pre, void* dx, int64_t n, int32_t act, cudaStream_t s) {
-  if (!dy || !pre || !dx) { set_error("act_bwd: null pointer"); return DVLA_ERR_INVALID; }
-  if (n <= 0) return DVLA_OK;
-  const bool vec = ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(pre) | reinterpret_cast<uintptr_t>(dx)) & 15) == 0;
-  long long blocks = ((vec ? (n + 7) / 8 : n) + 255) / 256;
-  if (blocks > 8LL * num_sms()) blocks = 8LL * num_sms();
-  if (vec) act_bwd_kernel<<<(unsigned)blocks, 256, 0, s>>>((const bf16*)dy, (const bf16*)pre, (bf16*)dx, n, act);
-  else     act_bwd_scalar_kernel<<<(unsigned)blocks, 256, 0, s>>>((const bf16*)dy, (const bf16*)pre, (bf16*)dx, n, act);
-  DVLA_CHECK_LAUNCH("act_bwd");
-  return DVLA_OK;
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -577,26 +466,6 @@ __global__ void __launch_bounds__(256) act_bwd_colsum_kernel(const bf16* __restr
   for (int w = 0; w < 8; ++w) t += red[w][c];
   if (blockIdx.x * 256 + c < N) atomicAdd(colsum + blockIdx.x * 256 + c, t);
 }
-int act_bwd_colsum_dispatch(const void* dy, const void* pre, void* dx, int64_t rows, int64_t N, int32_t act, float* colsum,
-                            cudaStream_t s) {
-  if (!dy || !pre || !dx || !colsum) { set_error("act_bwd_colsum: null pointer"); return DVLA_ERR_INVALID; }
-  if (rows <= 0 || N <= 0) return DVLA_OK;
-  if (N % 8 || ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(pre) | reinterpret_cast<uintptr_t>(dx)) & 15)) {
-    // unaligned / odd width: the two separate passes
-    int rc = act_bwd_dispatch(dy, pre, dx, rows * N, act, s);
-    if (rc != DVLA_OK) return rc;
-    return colsum_accum_dispatch(dx, rows, N, N, colsum, s);
-  }
-  const int bx = (int)((N + 255) / 256);
-  int by = (8 * num_sms() + bx - 1) / bx;
-  if (by > (rows + 31) / 32) by = (int)((rows + 31) / 32);
-  if (by < 1) by = 1;
-  const int rpb = (int)((rows + by - 1) / by);
-  by = (int)((rows + rpb - 1) / rpb);
-  act_bwd_colsum_kernel<<<dim3(bx, by), 256, 0, s>>>((const bf16*)dy, (const bf16*)pre, (bf16*)dx, rows, (int)N, colsum, rpb, act);
-  DVLA_CHECK_LAUNCH("act_bwd_colsum");
-  return DVLA_OK;
-}
 
 // ------------------------------------------------------------------------------------------------------------------
 // out[s, :a] = e[s], out[s, a:] = m: per-sequence rows followed by rows shared by every sequence (16-byte vectors)
@@ -613,7 +482,149 @@ __global__ void __launch_bounds__(256) cat_broadcast_kernel(const uint4* __restr
     out[i] = r < ea ? e[s * ea + r] : __ldg(m + (r - ea));
   }
 }
-int cat_broadcast_dispatch(const void* e, const void* m, void* out, int64_t n, int64_t a, int64_t b, int64_t C, cudaStream_t s) {
+
+}  // namespace dvla
+
+using namespace dvla;
+
+extern "C" int dvla_layernorm_fwd(const dvla_layernorm_fwd_args* a, void* stream) {
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  if (!a || !a->x || !a->y) { set_error("layernorm_fwd: null pointer"); return DVLA_ERR_INVALID; }
+  if (a->D % 8 || a->ldx % 8 || a->ldy % 8 || a->D > 1024 || a->D <= 0) {
+    set_error("layernorm_fwd: need D%%8==0, D<=1024, strides%%8==0 (D=%lld)", (long long)a->D);
+    return DVLA_ERR_UNSUPPORTED;
+  }
+  if (a->rows <= 0) return DVLA_OK;
+  const int nv = (int)((a->D + 255) / 256);
+  long long blocks = (a->rows + 7) / 8;
+  const long long cap = (long long)num_sms() * 8;
+  if (blocks > cap) blocks = cap;
+#define LN_FWD(NV) layernorm_fwd_kernel<NV><<<(unsigned)blocks, 256, 0, s>>>((const bf16*)a->x, (const bf16*)a->gamma, \
+      (const bf16*)a->beta, (bf16*)a->y, a->mean, a->rstd, a->rows, (int)a->D, a->ldx, a->ldy, a->eps)
+  switch (nv) { case 1: LN_FWD(1); break; case 2: LN_FWD(2); break; case 3: LN_FWD(3); break; default: LN_FWD(4); break; }
+#undef LN_FWD
+  DVLA_CHECK_LAUNCH("layernorm_fwd");
+  return DVLA_OK;
+}
+
+extern "C" int dvla_layernorm_bwd(const dvla_layernorm_bwd_args* a, void* stream) {
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  if (!a || !a->dy || !a->x || !a->mean || !a->rstd || !a->dx) { set_error("layernorm_bwd: null pointer"); return DVLA_ERR_INVALID; }
+  if (a->D % 8 || a->ld % 8 || a->D > 1024 || a->D <= 0) {
+    set_error("layernorm_bwd: need D%%8==0, D<=1024, ld%%8==0 (D=%lld)", (long long)a->D);
+    return DVLA_ERR_UNSUPPORTED;
+  }
+  if (a->rows <= 0) return DVLA_OK;
+  const int nv = (int)((a->D + 255) / 256);
+  long long blocks = (a->rows + 7) / 8;
+  if (a->D % 256 == 0 && (a->dgamma || a->dbeta) && a->rows >= 2048) {
+    const long long cap3 = 2LL * num_sms();
+    if (blocks > cap3) blocks = cap3;
+    const size_t smem = (size_t)8 * 2 * a->D * sizeof(float);
+#define LN_BWD2(NV) do { \
+      static const cudaError_t attr_e = cudaFuncSetAttribute(layernorm_bwd_v2_kernel<NV>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * 2 * NV * 256 * 4); \
+      if (attr_e != cudaSuccess) { set_error("layernorm_bwd_v2 smem attr: %s", cudaGetErrorString(attr_e)); return DVLA_ERR_CUDA; } \
+      layernorm_bwd_v2_kernel<NV><<<(unsigned)blocks, 256, smem, s>>>((const bf16*)a->dy, (const bf16*)a->x, (const bf16*)a->gamma, \
+          a->mean, a->rstd, (bf16*)a->dx, a->dgamma, a->dbeta, a->rows, a->ld, (const bf16*)a->dres); } while (0)
+    switch (nv) { case 1: LN_BWD2(1); break; case 2: LN_BWD2(2); break; case 3: LN_BWD2(3); break; default: LN_BWD2(4); break; }
+#undef LN_BWD2
+    DVLA_CHECK_LAUNCH("layernorm_bwd_v2");
+    return DVLA_OK;
+  }
+  const long long cap = 2LL * num_sms();        // 2 resident blocks per SM; 2*D fp32 atomics per block at the end
+  if (blocks > cap) blocks = cap;
+#define LN_BWD(NV) layernorm_bwd_kernel<NV><<<(unsigned)blocks, 256, 0, s>>>((const bf16*)a->dy, (const bf16*)a->x, \
+      (const bf16*)a->gamma, a->mean, a->rstd, (bf16*)a->dx, a->dgamma, a->dbeta, a->rows, (int)a->D, a->ld, (const bf16*)a->dres)
+  switch (nv) { case 1: LN_BWD(1); break; case 2: LN_BWD(2); break; case 3: LN_BWD(3); break; default: LN_BWD(4); break; }
+#undef LN_BWD
+  DVLA_CHECK_LAUNCH("layernorm_bwd");
+  return DVLA_OK;
+}
+
+extern "C" int dvla_colsum_accum(const void* x, int64_t rows, int64_t N, int64_t ld, float* out, void* stream) {
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  if (!x || !out) { set_error("colsum: null pointer"); return DVLA_ERR_INVALID; }
+  if (rows <= 0 || N <= 0) return DVLA_OK;
+  const int vec = (N % 8 == 0) && (ld % 8 == 0) && ((reinterpret_cast<uintptr_t>(x) & 15) == 0);
+  const int bx = (int)((N + 255) / 256);
+  int by = (int)((6LL * num_sms() + bx - 1) / bx);     // ~6 blocks of 256 threads per SM: enough loads in flight for HBM
+  if (by > (rows + 63) / 64) by = (int)((rows + 63) / 64);
+  if (by < 1) by = 1;
+  const int rpb = (int)((rows + by - 1) / by);
+  by = (int)((rows + rpb - 1) / rpb);
+  colsum_kernel<<<dim3(bx, by), 256, 0, s>>>((const bf16*)x, rows, (int)N, ld, out, rpb, vec);
+  DVLA_CHECK_LAUNCH("colsum");
+  return DVLA_OK;
+}
+
+extern "C" int dvla_accum_fp32_into_bf16(const float* src, void* dst, int64_t n, void* stream) {
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  if (!src || !dst) { set_error("accum_fp32_into_bf16: null pointer"); return DVLA_ERR_INVALID; }
+  if (n <= 0) return DVLA_OK;
+  long long blocks = (n + 255) / 256;
+  if (blocks > 4LL * num_sms()) blocks = 4LL * num_sms();
+  accum_fp32_into_bf16_kernel<<<(unsigned)blocks, 256, 0, s>>>(src, (bf16*)dst, n);
+  DVLA_CHECK_LAUNCH("accum_fp32_into_bf16");
+  return DVLA_OK;
+}
+
+extern "C" int dvla_dropout(const void* x, void* y, int64_t rows, int64_t N, int64_t ldx, int64_t ldy, float p, uint64_t seed,
+                            const uint64_t* seed_ptr, void* stream) {
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  if (!x || !y) { set_error("dropout: null pointer"); return DVLA_ERR_INVALID; }
+  if (!dropout_rate_ok(p)) { set_error("dropout: p out of range"); return DVLA_ERR_INVALID; }
+  if (rows <= 0 || N <= 0) return DVLA_OK;
+  uint32_t thresh;
+  float scale;
+  dropout_thresh_scale(p, &thresh, &scale);
+  const int vec = (N % 8 == 0) && (ldx % 8 == 0) && (ldy % 8 == 0) && ((reinterpret_cast<uintptr_t>(x) & 15) == 0) &&
+                  ((reinterpret_cast<uintptr_t>(y) & 15) == 0);
+  const long long total = rows * ((N + 7) / 8);
+  long long blocks = (total + 255) / 256;
+  if (blocks > 8LL * num_sms()) blocks = 8LL * num_sms();
+  dropout_kernel<<<(unsigned)blocks, 256, 0, s>>>((const bf16*)x, (bf16*)y, rows, (int)N, ldx, ldy, thresh, scale, seed, seed_ptr, vec);
+  DVLA_CHECK_LAUNCH("dropout");
+  return DVLA_OK;
+}
+
+extern "C" int dvla_act_bwd(const void* dy, const void* pre, void* dx, int64_t n, int32_t act, void* stream) {
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  if (!dy || !pre || !dx) { set_error("act_bwd: null pointer"); return DVLA_ERR_INVALID; }
+  if (n <= 0) return DVLA_OK;
+  const bool vec = ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(pre) | reinterpret_cast<uintptr_t>(dx)) & 15) == 0;
+  long long blocks = ((vec ? (n + 7) / 8 : n) + 255) / 256;
+  if (blocks > 8LL * num_sms()) blocks = 8LL * num_sms();
+  if (vec) act_bwd_kernel<<<(unsigned)blocks, 256, 0, s>>>((const bf16*)dy, (const bf16*)pre, (bf16*)dx, n, act);
+  else     act_bwd_scalar_kernel<<<(unsigned)blocks, 256, 0, s>>>((const bf16*)dy, (const bf16*)pre, (bf16*)dx, n, act);
+  DVLA_CHECK_LAUNCH("act_bwd");
+  return DVLA_OK;
+}
+
+extern "C" int dvla_act_bwd_colsum(const void* dy, const void* pre, void* dx, int64_t rows, int64_t N, int32_t act, float* colsum,
+                                   void* stream) {
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  if (!dy || !pre || !dx || !colsum) { set_error("act_bwd_colsum: null pointer"); return DVLA_ERR_INVALID; }
+  if (rows <= 0 || N <= 0) return DVLA_OK;
+  if (N % 8 || ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(pre) | reinterpret_cast<uintptr_t>(dx)) & 15)) {
+    // unaligned / odd width: the two separate passes
+    int rc = dvla_act_bwd(dy, pre, dx, rows * N, act, stream);
+    if (rc != DVLA_OK) return rc;
+    return dvla_colsum_accum(dx, rows, N, N, colsum, stream);
+  }
+  const int bx = (int)((N + 255) / 256);
+  int by = (8 * num_sms() + bx - 1) / bx;
+  if (by > (rows + 31) / 32) by = (int)((rows + 31) / 32);
+  if (by < 1) by = 1;
+  const int rpb = (int)((rows + by - 1) / by);
+  by = (int)((rows + rpb - 1) / rpb);
+  act_bwd_colsum_kernel<<<dim3(bx, by), 256, 0, s>>>((const bf16*)dy, (const bf16*)pre, (bf16*)dx, rows, (int)N, colsum, rpb, act);
+  DVLA_CHECK_LAUNCH("act_bwd_colsum");
+  return DVLA_OK;
+}
+
+extern "C" int dvla_cat_broadcast(const void* e, const void* m, void* out, int64_t n, int64_t a, int64_t b, int64_t C,
+                                  void* stream) {
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (!e || !m || !out) { set_error("cat_broadcast: null pointer"); return DVLA_ERR_INVALID; }
   if (n <= 0 || a < 0 || b <= 0 || C <= 0 || C % 8) { set_error("cat_broadcast: bad dims (C must be a multiple of 8)"); return DVLA_ERR_INVALID; }
   if ((reinterpret_cast<uintptr_t>(e) | reinterpret_cast<uintptr_t>(m) | reinterpret_cast<uintptr_t>(out)) & 15) {
@@ -627,5 +638,3 @@ int cat_broadcast_dispatch(const void* e, const void* m, void* out, int64_t n, i
   DVLA_CHECK_LAUNCH("cat_broadcast");
   return DVLA_OK;
 }
-
-}  // namespace dvla

@@ -38,7 +38,7 @@ def philox4x32(ctr, key, rounds=ROUNDS):
 
 
 def thresh_scale(p):
-    """(thresh, scale) exactly as the dispatchers round them from a float32 `p`."""
+    """(thresh, scale) exactly as the library rounds them from a float32 `p` (dropout_thresh_scale, csrc/host.cuh)."""
     pf = np.float32(p)
     thresh = int(np.uint32(pf * np.float32(65536.0) + np.float32(0.5)))
     scale = np.float32(1.0) / (np.float32(1.0) - np.float32(thresh) / np.float32(65536.0))

@@ -203,7 +203,7 @@ def _tmap_ok(t, L_):
 
 
 def attn_paths(q, k, v, d_o):
-    """Which kernels attn_fwd_dispatch / attn_bwd_dispatch pick with dropout on (the short-sequence kernels of
+    """Which kernels dvla_attn_fwd / dvla_attn_bwd pick with dropout on (the short-sequence kernels of
     attention_small.cu take no dropout): 'wgmma' or 'mma.sync' for the forward and for the backward."""
     Lq, Lk = q.shape[1], k.shape[1]
     fwd = Lq >= 96 and _tmap_ok(q, Lq) and _tmap_ok(k, Lk) and _tmap_ok(v, Lk)
