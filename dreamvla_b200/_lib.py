@@ -112,6 +112,7 @@ PROTOTYPES = {
     "dvla_attn_fwd": (_int, [_vp, _vp]),
     "dvla_attn_bwd": (_int, [_vp, _vp]),
     "dvla_attn_mask_tiles": (_int, [_vp, _i32, _i64, _i64, _vp, _vp]),
+    "dvla_attn_mask_obs_drop": (_int, [_vp, _vp, _vp, _i32, _i64, _i64, _i64, _i64, _i64, _i64, _i64, _u64, _vp, _vp]),
     "dvla_colsum_accum": (_int, [_vp, _i64, _i64, _i64, _vp, _vp]),
     "dvla_accum_fp32_into_bf16": (_int, [_vp, _vp, _i64, _vp]),
     "dvla_dropout": (_int, [_vp, _vp, _i64, _i64, _i64, _i64, _f32, _u64, _vp, _vp]),
@@ -334,11 +335,26 @@ def attn_bwd(q, k, v, o, d_o, lse, scale, dq, dk, dv, mask_bits=None, tile_flags
     _call("dvla_attn_bwd", C.byref(a), _stream())
 
 
-def attn_mask_tiles(mask_bits, Lq, Lk):
+def attn_mask_tiles(mask_bits, Lq, Lk, out=None):
+    """Tile flags [ceil(Lq/64), ceil(Lk/64)] uint8 of a bit mask; `out` refreshes an existing flags buffer in place."""
     nqt, nkt = (Lq + 63) // 64, (Lk + 63) // 64
-    flags = torch.empty((nqt, nkt), device=mask_bits.device, dtype=torch.uint8)
+    flags = torch.empty((nqt, nkt), device=mask_bits.device, dtype=torch.uint8) if out is None else out
+    assert flags.shape == (nqt, nkt) and flags.dtype == torch.uint8 and flags.is_contiguous()
     _call("dvla_attn_mask_tiles", mask_bits.data_ptr(), mask_bits.shape[1], Lq, Lk, flags.data_ptr(), _stream())
     return flags
+
+
+def attn_mask_obs_drop(base_bits, bits, flags, K, n_tok, num_A, n_obs, n_act, count, seed, seed_ptr=None):
+    """bits = base_bits with `count` observation columns per timestep hidden from that timestep's action rows, flags = its
+    tile flags (include/dvla.h dvla_attn_mask_obs_drop); both written in place, capturable in a CUDA graph."""
+    _need_cuda(base_bits, bits, flags, seed_ptr)
+    L_, W = base_bits.shape
+    assert bits.shape == (L_, W) and base_bits.dtype == bits.dtype == torch.int32
+    assert base_bits.is_contiguous() and bits.is_contiguous() and flags.is_contiguous() and flags.dtype == torch.uint8
+    assert flags.shape == ((L_ + 63) // 64, (L_ + 63) // 64)
+    assert seed_ptr is None or (seed_ptr.dtype == torch.int64 and seed_ptr.numel() >= 1)
+    _call("dvla_attn_mask_obs_drop", base_bits.data_ptr(), bits.data_ptr(), flags.data_ptr(), W, L_, K, n_tok, num_A, n_obs,
+          n_act, count, int(seed) & 0xFFFFFFFFFFFFFFFF, _ptr(seed_ptr), _stream())
 
 
 def colsum_accum(x2d, out_f32):

@@ -994,6 +994,47 @@ __global__ void attn_mask_tiles_kernel(const uint32_t* __restrict__ mask, int ma
   if (lane == 0) flags[tile] = any ? (all ? 2 : 1) : 0;
 }
 
+// ============================================ observation-token drop ==============================================
+// The pretrain phase's per-forward mask (dreamvla_model.py:55-59): for every timestep i, `count` of its n_obs observation
+// columns are hidden from that timestep's action rows.  Column j of timestep i draws the key r(i, j) =
+// philox4x32(seed + *seed_ptr, i * n_obs + j).x; the `count` columns with the smallest (r, j) are dropped -- a uniform
+// count-subset per timestep, independent across timesteps.  One block per timestep: rank every key against the others in
+// shared memory, then write the timestep's rows of `bits` = `base` with the dropped (action row, obs column) bits cleared.
+constexpr int OBS_DROP_THREADS = 256;
+constexpr int OBS_DROP_MAX_OBS = OBS_DROP_THREADS;
+
+__global__ void __launch_bounds__(OBS_DROP_THREADS)
+attn_mask_obs_drop_kernel(const uint32_t* __restrict__ base, uint32_t* __restrict__ bits, int mask_words, int n_tok,
+                          int num_A, int n_obs, int n_act, int count, uint64_t seed, const int64_t* __restrict__ seed_ptr) {
+  __shared__ uint64_t key[OBS_DROP_MAX_OBS];
+  __shared__ uint32_t span[OBS_DROP_MAX_OBS / 32 + 1];   // drop bits of the obs columns, aligned to the mask's words
+  const int i = blockIdx.x, t = threadIdx.x;
+  const uint64_t eff = seed + (seed_ptr ? static_cast<uint64_t>(*seed_ptr) : 0ull);
+  const int c0 = i * n_tok + num_A;                      // first observation column of timestep i
+  const int w0 = c0 >> 5, w1 = (c0 + n_obs - 1) >> 5;    // the words those columns span (n_obs >= 1)
+  if (t < n_obs) {
+    const uint32_t r = philox4x32(eff, static_cast<uint64_t>(i) * n_obs + t).x;
+    key[t] = (static_cast<uint64_t>(r) << 32) | static_cast<uint32_t>(t);   // distinct keys: ties broken by j
+  }
+  if (t <= w1 - w0) span[t] = 0u;
+  __syncthreads();
+  if (t < n_obs) {
+    const uint64_t mine = key[t];
+    int rank = 0;
+    for (int k = 0; k < n_obs; ++k) rank += key[k] < mine;
+    if (rank < count) atomicOr(&span[((c0 + t) >> 5) - w0], 1u << ((c0 + t) & 31));
+  }
+  __syncthreads();
+  const int a0 = num_A + n_obs;                          // first action row of the timestep, relative to its first row
+  const long long row0 = static_cast<long long>(i) * n_tok;
+  for (int e = t; e < n_tok * mask_words; e += OBS_DROP_THREADS) {
+    const int rr = e / mask_words, w = e - rr * mask_words;
+    uint32_t v = base[(row0 + rr) * mask_words + w];
+    if (rr >= a0 && rr < a0 + n_act && w >= w0 && w <= w1) v &= ~span[w - w0];
+    bits[(row0 + rr) * mask_words + w] = v;
+  }
+}
+
 // ===================================================== host =======================================================
 static bool strides_ok(const void* ptr, long long sb, long long ss, long long sh) {
   return ptr && (reinterpret_cast<uintptr_t>(ptr) % 16 == 0) && sb % 8 == 0 && ss % 8 == 0 && sh % 8 == 0;
@@ -1183,6 +1224,39 @@ extern "C" int dvla_attn_mask_tiles(const uint32_t* mask, int32_t mask_words, in
   attn_mask_tiles_kernel<<<(tiles + 3) / 4, 128, 0, s>>>(mask, mask_words, (int)Lq, (int)Lk, nkt, flags);
   DVLA_CHECK_LAUNCH("attn_mask_tiles");
   return DVLA_OK;
+}
+
+extern "C" int dvla_attn_mask_obs_drop(const uint32_t* base_bits, uint32_t* bits, uint8_t* tile_flags, int32_t mask_words,
+                                       int64_t L, int64_t K, int64_t n_tok, int64_t num_A, int64_t n_obs, int64_t n_act,
+                                       int64_t count, uint64_t seed, const int64_t* seed_ptr, void* stream) {
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  if (!base_bits || !bits || !tile_flags) { set_error("attn_mask_obs_drop: null pointer"); return DVLA_ERR_INVALID; }
+  if (base_bits == bits) { set_error("attn_mask_obs_drop: bits must not alias base_bits"); return DVLA_ERR_INVALID; }
+  if (L <= 0 || L > (1 << 24) || mask_words <= 0 || static_cast<int64_t>(mask_words) * 32 < L) {
+    set_error("attn_mask_obs_drop: L=%lld with mask_words=%d (need 0 < L <= 32 * mask_words)", (long long)L, (int)mask_words);
+    return DVLA_ERR_INVALID;
+  }
+  if (K <= 0 || n_tok <= 0 || K * n_tok != L) {
+    set_error("attn_mask_obs_drop: layout K=%lld x n_tok=%lld does not tile L=%lld", (long long)K, (long long)n_tok, (long long)L);
+    return DVLA_ERR_INVALID;
+  }
+  if (num_A < 0 || n_obs < 1 || n_act < 0 || num_A + n_obs + n_act > n_tok) {
+    set_error("attn_mask_obs_drop: num_A=%lld + n_obs=%lld + n_act=%lld outside n_tok=%lld (n_obs >= 1)", (long long)num_A,
+              (long long)n_obs, (long long)n_act, (long long)n_tok);
+    return DVLA_ERR_INVALID;
+  }
+  if (n_obs > OBS_DROP_MAX_OBS) {
+    set_error("attn_mask_obs_drop: n_obs=%lld above the kernel's limit of %d", (long long)n_obs, OBS_DROP_MAX_OBS);
+    return DVLA_ERR_INVALID;
+  }
+  if (count < 0 || count > n_obs) {
+    set_error("attn_mask_obs_drop: count=%lld outside [0, n_obs=%lld]", (long long)count, (long long)n_obs);
+    return DVLA_ERR_INVALID;
+  }
+  attn_mask_obs_drop_kernel<<<(unsigned)K, OBS_DROP_THREADS, 0, s>>>(base_bits, bits, mask_words, (int)n_tok, (int)num_A,
+                                                                     (int)n_obs, (int)n_act, (int)count, seed, seed_ptr);
+  DVLA_CHECK_LAUNCH("attn_mask_obs_drop");
+  return dvla_attn_mask_tiles(bits, mask_words, L, L, tile_flags, stream);
 }
 
 extern "C" int64_t dvla_attn_bwd_workspace_bytes(int64_t B, int64_t H, int64_t Lq) {

@@ -283,6 +283,7 @@ class DreamVLA(nn.Module):
         self.embedding_layer_norm = LayerNorm(D)
         self.attention_mask = nn.Parameter(self._make_mask(), requires_grad=False)
         self._mask_cache = None
+        self._obs_drop_seed = self._obs_drop_mask = None      # see obs_drop_on_device
         self.transformer_backbone_position_embedding = nn.Parameter(torch.zeros(1, sequence_length, 1, D), requires_grad=True)
         config = GPT2Config()
         config.hidden_size = D
@@ -388,14 +389,48 @@ class DreamVLA(nn.Module):
             return self.NUM_OBS_TOKEN + self.NUM_DEPTH_TOKEN + self.NUM_TRAJ_TOKEN + self.NUM_DINO_TOKEN + self.NUM_SAM_TOKEN
         return 0
 
-    def _make_mask(self):
+    def _make_mask(self, mask_l_obs_ratio=None):
         n_obs = self._this_num_obs_token()
+        ratio = self.mask_l_obs_ratio if mask_l_obs_ratio is None else mask_l_obs_ratio
         return generate_attention_mask(K=self.sequence_length, num_A=1 + 1 + self.NUM_RESAMPLER_QUERY * 2 + 1 * 2,
                                        num_B=n_obs + self.action_pred_steps, atten_goal=self.atten_goal,
                                        atten_goal_state=self.atten_goal_state, atten_only_obs=self.atten_only_obs,
                                        attn_robot_proprio_state=self.attn_robot_proprio_state,
-                                       mask_l_obs_ratio=self.mask_l_obs_ratio, num_obs_token=n_obs,
+                                       mask_l_obs_ratio=ratio, num_obs_token=n_obs,
                                        action_pred_steps=self.action_pred_steps)
+
+    @property
+    def redraws_mask(self):
+        """True when every training forward draws a fresh observation-token drop (reference :610-628 with :55-59)."""
+        return self.phase == "pretrain" and self.mask_l_obs_ratio > 0 and self.atten_only_obs
+
+    @property
+    def obs_drop_on_device(self):
+        """Whether a training forward that redraws the mask (`redraws_mask`) draws it on the device (ops.ObsDropMask, one
+        kernel, capturable in a CUDA graph) instead of through np.random on the host (the reference's call sequence, a
+        host-device round trip per forward).  Switching it on fixes the draw's seed from torch's default generator."""
+        return self._obs_drop_seed is not None
+
+    @obs_drop_on_device.setter
+    def obs_drop_on_device(self, on):
+        if not on:
+            self._obs_drop_seed = self._obs_drop_mask = None
+        elif not self.obs_drop_on_device:
+            self._obs_drop_seed = int(torch.randint(0, 2 ** 63 - 1, (1,)))
+            self._obs_drop_mask = None
+            if self.attention_mask.is_cuda:     # allocate now: the first draw may be inside a CUDA-graph capture
+                self._device_obs_drop(self.attention_mask.device)
+
+    def _device_obs_drop(self, device):
+        """The model's ops.ObsDropMask on `device`, built from the mask without the drop (mask_l_obs_ratio = 0)."""
+        m = self._obs_drop_mask
+        if m is None or m.bits.device != torch.device(device):
+            n_obs = self._this_num_obs_token()
+            m = self._obs_drop_mask = ops.ObsDropMask(
+                self._make_mask(mask_l_obs_ratio=0.0) == 0, device, K=self.sequence_length,
+                num_A=1 + 1 + self.NUM_RESAMPLER_QUERY * 2 + 1 * 2, n_obs=n_obs, n_act=self.action_pred_steps,
+                count=int(self.mask_l_obs_ratio * n_obs), seed=self._obs_drop_seed)      # count as the reference's (:57)
+        return m
 
     def _attn_mask(self, device):
         """Bit-matrix form of self.attention_mask, rebuilt when the parameter changes (pretrain phase / load_state_dict)."""
@@ -620,7 +655,8 @@ class DreamVLA(nn.Module):
                 mode="train", diffusion_noise=None, diffusion_timestep=None, diffusion_drop_ids=None, sample_noise=None):
         """Reference :609-991.  The four trailing keyword arguments inject the tensors the reference samples inside
         forward (action_model.py:59-60, models.py:83, dreamvla_model.py:944) so parity tests can line them up."""
-        if self.training and self.phase == "pretrain" and self.mask_l_obs_ratio > 0 and self.atten_only_obs:
+        device_drop = self.training and self.redraws_mask and self.obs_drop_on_device
+        if self.training and self.redraws_mask and not device_drop:
             # :610-628 mask regenerated each forward; only the np.random column drop (:55-59) makes it differ
             self.attention_mask = nn.Parameter(self._make_mask().to(self.attention_mask.device), requires_grad=False)
         B, S, _ = state.shape
@@ -661,7 +697,9 @@ class DreamVLA(nn.Module):
         transformer_input = self.embedding_layer_norm(transformer_input)
         marks = getattr(self, "_dvla_grad_marks", None)      # set by TrainStep: overlap the gradient all-reduce with backward
         self.transformer_backbone._dvla_grad_mark = marks["backbone_cuts"] if marks else None
-        transformer_output = self.transformer_backbone(inputs_embeds=transformer_input, attention_mask=self._attn_mask(dev))
+        # device draw: one per forward, TrainStep advances the seed counter every micro-step (also under CUDA-graph replay)
+        mask = self._device_obs_drop(dev).draw(ops.seed_counter(dev)) if device_drop else self._attn_mask(dev)
+        transformer_output = self.transformer_backbone(inputs_embeds=transformer_input, attention_mask=mask)
         if marks and transformer_output.requires_grad:
             ops.on_grad_ready(transformer_output, marks["backbone_out"])
         transformer_output = transformer_output.view(B, S, -1, D)

@@ -333,6 +333,25 @@ class AttnMask:
         return AttnMask(torch.ones(n, n, dtype=torch.bool).tril(), device)
 
 
+class ObsDropMask(AttnMask):
+    """AttnMask redrawn on the device: every draw() hides `count` of each timestep's n_obs observation columns from that
+    timestep's action rows (the pretrain phase's per-forward drop, dreamvla_model.py:55-59), writing `bits` and `flags` in
+    place.  Buffers are allocated once and nothing is read back, so a draw can be captured in a CUDA graph; the attention ops
+    of a forward and its backward read the same buffers.  Draw rule: include/dvla.h dvla_attn_mask_obs_drop."""
+
+    def __init__(self, base_visible: torch.Tensor, device, K: int, num_A: int, n_obs: int, n_act: int, count: int, seed: int):
+        super().__init__(base_visible, device)
+        self.base_bits = self.bits.clone()
+        self.layout = (K, self.Lq // K, num_A, n_obs, n_act, count)
+        self.seed = int(seed)
+
+    def draw(self, seed_ptr: torch.Tensor):
+        """Redraw under the effective seed `seed + *seed_ptr` (seed_ptr: device int64 counter, ops.seed_counter)."""
+        if self.layout[3] > 0:          # no observation tokens: nothing to drop, the base mask stands
+            L.attn_mask_obs_drop(self.base_bits, self.bits, self.flags, *self.layout, self.seed, seed_ptr)
+        return self
+
+
 class _CatBroadcast(torch.autograd.Function):
     """[n, a, C] per-sequence rows + [b, C] rows shared by every sequence -> [n, a + b, C]; the gradient of the shared rows
     is the sum over sequences (column-sum kernel over the [n, b*C] view of the incoming gradient)."""

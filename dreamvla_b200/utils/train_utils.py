@@ -595,6 +595,9 @@ class GraphedTrainStep:
                              "reduce_every_micro_step=False and world_size > 1 use gradient_accumulation_steps == 1 or the "
                              "eager TrainStep")
         self.step = step
+        if getattr(step.model, "redraws_mask", False):
+            # the host draw of the pretrain mask (np.random + a device-to-host read) cannot be captured: draw it on the device
+            step.model.obs_drop_on_device = True
         self.static = {k: v.clone() for k, v in example_batch.items()}
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())

@@ -182,6 +182,18 @@ int dvla_attn_bwd(const dvla_attn_bwd_args* args, void* stream);
 int dvla_attn_mask_tiles(const uint32_t* mask, int32_t mask_words, int64_t Lq, int64_t Lk, uint8_t* tile_flags,
                          void* stream);
 
+/* The pretrain phase's per-forward observation-token drop (dreamvla_model.py:55-59), drawn on the device.
+ * base_bits [L, mask_words]: the mask built with mask_l_obs_ratio = 0; layout: K timesteps of n_tok slots each (K*n_tok = L),
+ * slots [num_A, num_A + n_obs) of a timestep are its observation tokens and the n_act slots after them its action tokens.
+ * For timestep i and observation column j < n_obs the key is r(i, j) = philox4x32(seed + *seed_ptr, i*n_obs + j).x (word 0,
+ * the 7-round Philox of the dropout masks; seed_ptr NULL counts as 0); the `count` columns with the smallest (r(i, j), j) are
+ * dropped: bits (action rows of i) x (column i*n_tok + num_A + j) are cleared.  bits = base_bits otherwise (must not alias).
+ * tile_flags [ceil(L/64), ceil(L/64)] is rebuilt from bits as by dvla_attn_mask_tiles.  No host reads, no allocation: the
+ * call can be captured in a CUDA graph.  n_obs <= 256 and 0 <= count <= n_obs, else DVLA_ERR_INVALID. */
+int dvla_attn_mask_obs_drop(const uint32_t* base_bits, uint32_t* bits, uint8_t* tile_flags, int32_t mask_words, int64_t L,
+                            int64_t K, int64_t n_tok, int64_t num_A, int64_t n_obs, int64_t n_act, int64_t count,
+                            uint64_t seed, const int64_t* seed_ptr, void* stream);
+
 /* ---------------------------------------------------------------------------------------------------------------
  * Element-wise / reduction helpers
  * ------------------------------------------------------------------------------------------------------------- */
