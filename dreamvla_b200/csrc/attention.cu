@@ -11,6 +11,8 @@
 //   attn_bwd_dkv_kernel grid (ceil(Lk/64), H, B): per key tile, loops over query tiles, S^T/dP^T formulation
 //   attn_bwd_dq_kernel  grid (ceil(Lq/64), H, B): per query tile, loops over key tiles
 // Masking: tile_flags[qt, kt] in {0 skip, 1 partial, 2 full}; partial tiles test bits of mask[i, j/32].
+// Both kernel families share the per-fragment helpers below dropout_bits: mask words, the forward tile step, the dQ-form dS
+// and the scaled bf16 store.  The forward finish and the dK/dV-form P / dS^T stay written out per kernel (see there).
 #include <string.h>
 
 #include <mutex>
@@ -32,7 +34,6 @@ struct AttnParams {
   const uint32_t* mask;
   const uint8_t* tile_flags;
   int B, H, Lq, Lk, nqt, nkt, mask_words;
-  int qt0, kt0;          // first q / kv 64-row tile of this launch
   long long q_sb, q_ss, q_sh, k_sb, k_ss, k_sh, v_sb, v_ss, v_sh, o_sb, o_ss, o_sh;
   long long do_sb, do_ss, do_sh, dq_sb, dq_ss, dq_sh, dk_sb, dk_ss, dk_sh, dv_sb, dv_ss, dv_sh;
   float scale;
@@ -164,8 +165,8 @@ __device__ __forceinline__ void dropout_bits(const AttnParams& p, long long bh, 
       keep[t] = ((m0 >> (2 * c)) & 3u) | (((m1 >> (2 * c)) & 3u) << 2);
     }
   } else {
-    // rows = keys (g, g+8 -> same 8-key RNG block iff ... no: keys g and g+8 are in different blocks), cols = queries.
-    // element (key kr, query qc): block = (bh*Lq + qc) * nblk + kr/8, bit kr%8.
+    // rows = keys, cols = queries: a block holds 8 keys of one query, and keys g and g+8 lie in different blocks, so each
+    // of a thread's 32 elements draws its own block.  Element (key kr, query qc): block (bh*Lq + qc) * nblk + kr/8, bit kr%8.
 #pragma unroll
     for (int t = 0; t < 8; ++t) {
       uint32_t bits = 0;
@@ -181,11 +182,139 @@ __device__ __forceinline__ void dropout_bits(const AttnParams& p, long long bh, 
   }
 }
 
+// ---- per-fragment attention math, shared by the mma.sync and the wgmma kernels -----------------------------------------
+// A warp's 16 x 64 fp32 fragment f[t][e] -- an mma.sync C fragment, or the warp's part of a wgmma m64n64 accumulator, which
+// has the same layout (common.cuh) -- holds row row0 + lane/4 + 8*(e/2), column col0 + 8t + 2*(lane%4) + e%2.
+// sc = scale * log2(e) is passed in: the callers compute it once before their tile loop (computed per tile inside
+// fwd_tile_step, it made the wgmma forward ~1.5% slower at the ViT shape on an H100).
+
+// Mask words of the query rows row0 + lane/4 + {0, 8} over keys [k0, k0 + 64): all ones unless the tile is partial (flag 1).
+__device__ __forceinline__ void row_mask_words(const AttnParams& p, int row0, int k0, int flag, uint32_t (&w)[2][2]) {
+  const int g = (threadIdx.x & 31) >> 2;
+  w[0][0] = w[0][1] = w[1][0] = w[1][1] = 0xffffffffu;
+  if (flag != 1) return;
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int row = row0 + g + r * 8;
+#pragma unroll
+    for (int ww = 0; ww < 2; ++ww) {
+      const int wi = (k0 >> 5) + ww;
+      w[r][ww] = (row < p.Lq && wi < p.mask_words) ? p.mask[static_cast<long long>(row) * p.mask_words + wi] : 0u;
+    }
+  }
+}
+
+// Forward step over the key tile [k0, k0 + 64) on S = Q K^T (rows = queries from row0): hide the keys the mask (flag 1) or
+// the sequence end hides, scale by sc into the log2 domain, fold the tile into the online softmax (m_run, l_run, o
+// rescaled) and drop elements of P.  Leaves P in s.
+__device__ __forceinline__ void fwd_tile_step(const AttnParams& p, float sc, long long bh, int row0, int k0, int flag,
+                                              float (&s)[8][4], float (&o)[8][4], float (&m_run)[2], float (&l_run)[2]) {
+  const int c = threadIdx.x & 3;
+  const bool tail = (k0 + 64 > p.Lk);
+  uint32_t w[2][2];
+  row_mask_words(p, row0, k0, flag, w);
+  float tmax[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+  for (int t = 0; t < 8; ++t) {
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int r = e >> 1;
+      const int kk = t * 8 + 2 * c + (e & 1);
+      bool vis = true;
+      if (flag == 1) vis = (w[r][kk >> 5] >> (kk & 31)) & 1u;
+      if (tail) vis = vis && (k0 + kk < p.Lk);
+      const float v = vis ? s[t][e] * sc : -INFINITY;
+      s[t][e] = v;
+      tmax[r] = fmaxf(tmax[r], v);
+    }
+  }
+  float alpha[2], muse[2];
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const float mn = fmaxf(m_run[r], quad_max(tmax[r]));
+    muse[r] = (mn == -INFINITY) ? 0.f : mn;
+    alpha[r] = exp2f(m_run[r] - muse[r]);
+    m_run[r] = mn;
+    l_run[r] *= alpha[r];
+  }
+#pragma unroll
+  for (int t = 0; t < 8; ++t) {
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int r = e >> 1;
+      const float pv = exp2f(s[t][e] - muse[r]);
+      s[t][e] = pv;
+      l_run[r] += pv;
+      o[t][e] *= alpha[r];
+    }
+  }
+  if (p.drop_scale != 0.f) {
+    uint32_t keep[8];
+    dropout_bits(p, bh, row0, k0, false, keep);
+#pragma unroll
+    for (int t = 0; t < 8; ++t)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) s[t][e] = ((keep[t] >> e) & 1u) ? s[t][e] * p.drop_scale : 0.f;
+  }
+}
+
+// lse * log2(e) and delta of the query rows row0 + lane/4 + {0, 8}; +inf and 0 past Lq, so that those rows get P = 0.
+__device__ __forceinline__ void row_lse_delta(const AttnParams& p, long long bh, int row0, float (&lse2)[2], float (&dlt)[2]) {
+  const int g = (threadIdx.x & 31) >> 2;
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int row = row0 + g + r * 8;
+    lse2[r] = (row < p.Lq) ? p.lse[bh * p.Lq + row] * LOG2E : INFINITY;
+    dlt[r] = (row < p.Lq) ? p.delta[bh * p.Lq + row] : 0.f;
+  }
+}
+
+// dS = P o (dP - delta) over the key tile [k0, k0 + 64), rows = queries from row0 with their row_lse_delta: P recomputed
+// from the LSE and sc, dP dropped with the forward's mask.  Leaves dS in s.
+__device__ __forceinline__ void dq_form_ds(const AttnParams& p, float sc, long long bh, int row0, int k0, int flag,
+                                           const float (&lse2)[2], const float (&dlt)[2], float (&s)[8][4],
+                                           const float (&dp)[8][4]) {
+  const int c = threadIdx.x & 3;
+  uint32_t w[2][2];
+  row_mask_words(p, row0, k0, flag, w);
+  uint32_t keep[8];
+  if (p.drop_scale != 0.f) dropout_bits(p, bh, row0, k0, false, keep);
+#pragma unroll
+  for (int t = 0; t < 8; ++t) {
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int r = e >> 1;
+      const int kk = t * 8 + 2 * c + (e & 1);
+      bool vis = (k0 + kk < p.Lk);
+      if (flag == 1) vis = vis && ((w[r][kk >> 5] >> (kk & 31)) & 1u);
+      const float pv = vis ? exp2f(s[t][e] * sc - lse2[r]) : 0.f;
+      float dpv = dp[t][e];
+      if (p.drop_scale != 0.f) dpv = ((keep[t] >> e) & 1u) ? dpv * p.drop_scale : 0.f;
+      s[t][e] = pv * (dpv - dlt[r]);
+    }
+  }
+}
+
+// Rows row0 + lane/4 + {0, 8} of a fragment times `scale`, as bf16 at dst + row * ss; rows >= L are not stored.
+__device__ __forceinline__ void store_frag_bf16(bf16* dst, long long ss, int row0, int L, const float (&f)[8][4], float scale) {
+  const int lane = threadIdx.x & 31, g = lane >> 2, c = lane & 3;
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int row = row0 + g + r * 8;
+    if (row < L) {
+      bf16* d = dst + static_cast<long long>(row) * ss;
+#pragma unroll
+      for (int t = 0; t < 8; ++t)
+        *reinterpret_cast<uint32_t*>(d + t * 8 + 2 * c) = pack_bf16x2(f[t][2 * r] * scale, f[t][2 * r + 1] * scale);
+    }
+  }
+}
+
 // ===================================================== forward ====================================================
 __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnParams p) {
   __shared__ __align__(1024) uint8_t sm[5 * 8192];
   const uint32_t sQ = smem_u32(sm), sK0 = sQ + 8192, sV0 = sQ + 2 * 8192, sK1 = sQ + 3 * 8192, sV1 = sQ + 4 * 8192;
-  const int qt = blockIdx.x + p.qt0, h = blockIdx.y, b = blockIdx.z;
+  const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, c = lane & 3;
   const int q0 = qt * 64;
   const bf16* qg = p.q + b * p.q_sb + h * p.q_sh;
@@ -231,66 +360,7 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnParams p) {
     float s[8][4];
     zero_c(s);
     mma_a_tT(s, qf, sK);
-
-    // ---- mask + scale (log2 domain) ----
-    const int flag = flags ? flags[kt] : 2;
-    const int k0 = kt * 64;
-    const bool tail = (k0 + 64 > p.Lk);
-    uint32_t w[2][2] = {{0xffffffffu, 0xffffffffu}, {0xffffffffu, 0xffffffffu}};
-    if (flag == 1) {
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        const int row = q0 + warp * 16 + g + r * 8;
-#pragma unroll
-        for (int ww = 0; ww < 2; ++ww) {
-          const int wi = kt * 2 + ww;
-          w[r][ww] = (row < p.Lq && wi < p.mask_words) ? p.mask[static_cast<long long>(row) * p.mask_words + wi] : 0u;
-        }
-      }
-    }
-    float tmax[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-    for (int t = 0; t < 8; ++t) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int r = e >> 1;
-        const int kk = t * 8 + 2 * c + (e & 1);
-        bool vis = true;
-        if (flag == 1) vis = (w[r][kk >> 5] >> (kk & 31)) & 1u;
-        if (tail) vis = vis && (k0 + kk < p.Lk);
-        const float v = vis ? s[t][e] * sc : -INFINITY;
-        s[t][e] = v;
-        tmax[r] = fmaxf(tmax[r], v);
-      }
-    }
-    float alpha[2], muse[2];
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      const float mn = fmaxf(m_run[r], quad_max(tmax[r]));
-      muse[r] = (mn == -INFINITY) ? 0.f : mn;
-      alpha[r] = exp2f(m_run[r] - muse[r]);
-      m_run[r] = mn;
-      l_run[r] *= alpha[r];
-    }
-#pragma unroll
-    for (int t = 0; t < 8; ++t) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int r = e >> 1;
-        const float pv = exp2f(s[t][e] - muse[r]);
-        s[t][e] = pv;
-        l_run[r] += pv;
-        o[t][e] *= alpha[r];
-      }
-    }
-    if (p.drop_scale != 0.f) {
-      uint32_t keep[8];
-      dropout_bits(p, bh, q0 + warp * 16, k0, false, keep);
-#pragma unroll
-      for (int t = 0; t < 8; ++t)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) s[t][e] = ((keep[t] >> e) & 1u) ? s[t][e] * p.drop_scale : 0.f;
-    }
+    fwd_tile_step(p, sc, bh, q0 + warp * 16, kt * 64, flags ? flags[kt] : 2, s, o, m_run, l_run);
     uint32_t pa[4][4];
     c_to_a(s, pa);
     mma_p_t(o, pa, sV);
@@ -300,7 +370,7 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnParams p) {
   }
   cp_async_wait<0>();
 
-  // ---- finalize ----
+  // ---- finalize (repeated in attn_fwd_wgmma_kernel: as a shared helper it cost this kernel a register) ----
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     const float l = quad_sum(l_run[r]);
@@ -320,8 +390,8 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnParams p) {
 // Warp-specialised forward for sequences of >= 96 queries.  CTA = 288 threads over the q-tiles 2x and 2x+1 (64 queries
 // each) of one (b, h):
 //   warps 0-3 / 4-7  consumer warpgroup g: S = Q_g K^T (wgmma m64n64k16, both operands from smem), mask / online softmax /
-//                    dropout in registers (the per-warp accumulator layout equals mma.sync's C fragment, so the code below
-//                    is that of attn_fwd_kernel), P -> bf16 register A operand, O += P V (wgmma, V read MN-major)
+//                    dropout in registers (fwd_tile_step on each warp's part of the accumulator), P -> bf16 register A
+//                    operand, O += P V (wgmma, V read MN-major)
 //   warp 8           TMA producer (one thread): Q of both tiles once, then K/V tiles of 64 keys through a 3-stage ring
 //                    (mbarrier tx); a K/V tile is loaded when either q-tile sees part of it, and both groups release it.
 // 4-D tensor maps (d, seq|head, head|seq, batch) address q/k/v in place in the fused QKV buffer; rows past L are zero.
@@ -397,7 +467,6 @@ __global__ void __launch_bounds__(WF_THREADS, 2) attn_fwd_wgmma_kernel(const __g
   // -------------------------------------------------- consumers ---------------------------------------------------
   const int g = warp >> 2, wq = warp & 3;         // consumer group (q-tile qt_base + g), warp within the group
   const int qt = qt_base + g, q0 = qt * 64;
-  const int c = lane & 3, gr = lane >> 2;
   const uint8_t* flags = fl0 ? fl0 + g * p.nkt : nullptr;
   const long long bh = static_cast<long long>(b) * p.H + h;
   const float sc = p.scale * LOG2E;
@@ -422,65 +491,7 @@ __global__ void __launch_bounds__(WF_THREADS, 2) attn_fwd_wgmma_kernel(const __g
       wgmma_commit();
       wgmma_wait<0>();
       wgmma_fence_operand32(sd);
-
-      // ---- mask + scale (log2 domain), as attn_fwd_kernel ----
-      const int k0 = kt * 64;
-      const bool tail = (k0 + 64 > p.Lk);
-      uint32_t w[2][2] = {{0xffffffffu, 0xffffffffu}, {0xffffffffu, 0xffffffffu}};
-      if (flag == 1) {
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-          const int row = q0 + wq * 16 + gr + r * 8;
-#pragma unroll
-          for (int ww = 0; ww < 2; ++ww) {
-            const int wi = kt * 2 + ww;
-            w[r][ww] = (row < p.Lq && wi < p.mask_words) ? p.mask[static_cast<long long>(row) * p.mask_words + wi] : 0u;
-          }
-        }
-      }
-      float tmax[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-      for (int t = 0; t < 8; ++t) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int r = e >> 1;
-          const int kk = t * 8 + 2 * c + (e & 1);
-          bool vis = true;
-          if (flag == 1) vis = (w[r][kk >> 5] >> (kk & 31)) & 1u;
-          if (tail) vis = vis && (k0 + kk < p.Lk);
-          const float v = vis ? s[t][e] * sc : -INFINITY;
-          s[t][e] = v;
-          tmax[r] = fmaxf(tmax[r], v);
-        }
-      }
-      float alpha[2], muse[2];
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        const float mn = fmaxf(m_run[r], quad_max(tmax[r]));
-        muse[r] = (mn == -INFINITY) ? 0.f : mn;
-        alpha[r] = exp2f(m_run[r] - muse[r]);
-        m_run[r] = mn;
-        l_run[r] *= alpha[r];
-      }
-#pragma unroll
-      for (int t = 0; t < 8; ++t) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int r = e >> 1;
-          const float pv = exp2f(s[t][e] - muse[r]);
-          s[t][e] = pv;
-          l_run[r] += pv;
-          o[t][e] *= alpha[r];
-        }
-      }
-      if (p.drop_scale != 0.f) {
-        uint32_t keep[8];
-        dropout_bits(p, bh, q0 + wq * 16, k0, false, keep);
-#pragma unroll
-        for (int t = 0; t < 8; ++t)
-#pragma unroll
-          for (int e = 0; e < 4; ++e) s[t][e] = ((keep[t] >> e) & 1u) ? s[t][e] * p.drop_scale : 0.f;
-      }
+      fwd_tile_step(p, sc, bh, q0 + wq * 16, kt * 64, flag, s, o, m_run, l_run);
       uint32_t pa[4][4];
       c_to_a(s, pa);
       float (&od)[32] = *reinterpret_cast<float(*)[32]>(&o[0][0]);
@@ -498,6 +509,7 @@ __global__ void __launch_bounds__(WF_THREADS, 2) attn_fwd_wgmma_kernel(const __g
   if (g == 1 && !has1) return;
 
   // ---- finalize, as attn_fwd_kernel ----
+  const int c = lane & 3, gr = lane >> 2;
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     const float l = quad_sum(l_run[r]);
@@ -545,7 +557,7 @@ __global__ void __launch_bounds__(128) attn_bwd_dkv_kernel(const AttnParams p) {
   __shared__ float s_lse[64], s_delta[64];
   __shared__ uint32_t s_mask[64][2];
   const uint32_t sK = smem_u32(sm), sV = sK + 8192, sQ = sK + 2 * 8192, sDO = sK + 3 * 8192;
-  const int kt = blockIdx.x + p.kt0, h = blockIdx.y, b = blockIdx.z;
+  const int kt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, c = lane & 3;
   const int k0 = kt * 64;
   const bf16* qg = p.q + b * p.q_sb + h * p.q_sh;
@@ -630,28 +642,16 @@ __global__ void __launch_bounds__(128) attn_bwd_dkv_kernel(const AttnParams p) {
     c_to_a(st, pa);
     mma_p_t(dk, pa, sQ);    // dK += dS^T * Q
   }
-
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const int key = k0 + warp * 16 + g + r * 8;
-    if (key < p.Lk) {
-      bf16* dkd = p.dk + b * p.dk_sb + static_cast<long long>(key) * p.dk_ss + h * p.dk_sh;
-      bf16* dvd = p.dv + b * p.dv_sb + static_cast<long long>(key) * p.dv_ss + h * p.dv_sh;
-#pragma unroll
-      for (int t = 0; t < 8; ++t) {
-        *reinterpret_cast<uint32_t*>(dkd + t * 8 + 2 * c) = pack_bf16x2(dk[t][2 * r] * p.scale, dk[t][2 * r + 1] * p.scale);
-        *reinterpret_cast<uint32_t*>(dvd + t * 8 + 2 * c) = pack_bf16x2(dv[t][2 * r], dv[t][2 * r + 1]);
-      }
-    }
-  }
+  store_frag_bf16(p.dk + b * p.dk_sb + h * p.dk_sh, p.dk_ss, k0 + warp * 16, p.Lk, dk, p.scale);
+  store_frag_bf16(p.dv + b * p.dv_sb + h * p.dv_sh, p.dv_ss, k0 + warp * 16, p.Lk, dv, 1.f);
 }
 
 // ===================================================== dQ =========================================================
 __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const AttnParams p) {
   __shared__ __align__(1024) uint8_t sm[4 * 8192];
   const uint32_t sQ = smem_u32(sm), sDO = sQ + 8192, sK = sQ + 2 * 8192, sV = sQ + 3 * 8192;
-  const int qt = blockIdx.x + p.qt0, h = blockIdx.y, b = blockIdx.z;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, c = lane & 3;
+  const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int warp = threadIdx.x >> 5;
   const int q0 = qt * 64;
   const bf16* qg = p.q + b * p.q_sb + h * p.q_sh;
   const bf16* kg = p.k + b * p.k_sb + h * p.k_sh;
@@ -670,12 +670,7 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const AttnParams p) {
   load_a_frags(sQ, warp * 16, qf);
   load_a_frags(sDO, warp * 16, dof);
   float lse2[2], dlt[2];
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const int row = q0 + warp * 16 + g + r * 8;
-    lse2[r] = (row < p.Lq) ? p.lse[bh * p.Lq + row] * LOG2E : INFINITY;
-    dlt[r] = (row < p.Lq) ? p.delta[bh * p.Lq + row] : 0.f;
-  }
+  row_lse_delta(p, bh, q0 + warp * 16, lse2, dlt);
   float dq[8][4];
   zero_c(dq);
 
@@ -696,54 +691,17 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const AttnParams p) {
     float dp[8][4];
     zero_c(dp);
     mma_a_tT(dp, dof, sV);     // dP = dO V^T
-
-    uint32_t w[2][2] = {{0xffffffffu, 0xffffffffu}, {0xffffffffu, 0xffffffffu}};
-    if (flag == 1) {
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        const int row = q0 + warp * 16 + g + r * 8;
-#pragma unroll
-        for (int ww = 0; ww < 2; ++ww) {
-          const int wi = kt * 2 + ww;
-          w[r][ww] = (row < p.Lq && wi < p.mask_words) ? p.mask[static_cast<long long>(row) * p.mask_words + wi] : 0u;
-        }
-      }
-    }
-    uint32_t keep[8];
-    if (p.drop_scale != 0.f) dropout_bits(p, bh, q0 + warp * 16, k0, false, keep);
-#pragma unroll
-    for (int t = 0; t < 8; ++t) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int r = e >> 1;
-        const int kk = t * 8 + 2 * c + (e & 1);
-        bool vis = (k0 + kk < p.Lk);
-        if (flag == 1) vis = vis && ((w[r][kk >> 5] >> (kk & 31)) & 1u);
-        const float pv = vis ? exp2f(s[t][e] * sc - lse2[r]) : 0.f;
-        float dpv = dp[t][e];
-        if (p.drop_scale != 0.f) dpv = ((keep[t] >> e) & 1u) ? dpv * p.drop_scale : 0.f;
-        s[t][e] = pv * (dpv - dlt[r]);   // dS
-      }
-    }
+    dq_form_ds(p, sc, bh, q0 + warp * 16, k0, flag, lse2, dlt, s, dp);
     uint32_t pa[4][4];
     c_to_a(s, pa);
     mma_p_t(dq, pa, sK);       // dQ += dS K
   }
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const int row = q0 + warp * 16 + g + r * 8;
-    if (row < p.Lq) {
-      bf16* dst = p.dq + b * p.dq_sb + static_cast<long long>(row) * p.dq_ss + h * p.dq_sh;
-#pragma unroll
-      for (int t = 0; t < 8; ++t)
-        *reinterpret_cast<uint32_t*>(dst + t * 8 + 2 * c) = pack_bf16x2(dq[t][2 * r] * p.scale, dq[t][2 * r + 1] * p.scale);
-    }
-  }
+  store_frag_bf16(p.dq + b * p.dq_sb + h * p.dq_sh, p.dq_ss, q0 + warp * 16, p.Lq, dq, p.scale);
 }
 
 // ============================================ backward, wgmma + TMA ================================================
 // Warp-specialised backward for sequences of >= 96 on both sides, in the S^T / dP^T formulation of attn_bwd_dkv_kernel and
-// the S / dP one of attn_bwd_dq_kernel (same masking, LSE recompute and dropout regeneration):
+// the S / dP one of attn_bwd_dq_kernel (dq_form_ds):
 //   DKV = true : CTA = key tiles 2x, 2x+1 of one (b, h); consumer group g owns key tile 2x+g (K, V loaded once) and streams
 //                query tiles (Q, dO): S^T = K Q^T, dP^T = V dO^T (wgmma, smem x smem), dV += P^T dO, dK += dS^T Q (wgmma,
 //                register A operand, Q / dO read MN-major)
@@ -820,14 +778,7 @@ __global__ void __launch_bounds__(WF_THREADS, 1) attn_bwd_wgmma_kernel(const __g
   zero_c(acc0);
   zero_c(acc1);
   float lse2[2], dlt[2];
-  if (!DKV) {
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      const int row = f0 + wq * 16 + gr + r * 8;
-      lse2[r] = (row < p.Lq) ? p.lse[bh * p.Lq + row] * LOG2E : INFINITY;
-      dlt[r] = (row < p.Lq) ? p.delta[bh * p.Lq + row] : 0.f;
-    }
-  }
+  if (!DKV) row_lse_delta(p, bh, f0 + wq * 16, lse2, dlt);
   mbar_wait<false>(f_full, 0);
 
   int st = 0; uint32_t ph = 0;
@@ -851,10 +802,11 @@ __global__ void __launch_bounds__(WF_THREADS, 1) attn_bwd_wgmma_kernel(const __g
       wgmma_wait<0>();
       wgmma_fence_operand32(sd);
       wgmma_fence_operand32(dpd);
-      uint32_t keep[8];
       if (DKV) {
-        // ---- as attn_bwd_dkv_kernel: rows = keys (f0 + ...), cols = queries (s0r + ...) ----
+        // ---- as attn_bwd_dkv_kernel: rows = keys (f0 + ...), cols = queries (s0r + ...).  Not shared with it: a
+        // helper taking the query's lse / delta / mask word through lambdas made this kernel 2.5-4% slower on an H100 ----
         const int k0 = f0, q0 = s0r;
+        uint32_t keep[8];
         if (p.drop_scale != 0.f) dropout_bits(p, bh, k0 + wq * 16, q0, true, keep);
         const int ww = wq >> 1;                               // mask word of this warp's 16 key rows
         float pt[8][4];
@@ -900,35 +852,8 @@ __global__ void __launch_bounds__(WF_THREADS, 1) attn_bwd_wgmma_kernel(const __g
         wgmma_fence_operand32(dkd);
         wgmma_fence_operand32(dvd);
       } else {
-        // ---- as attn_bwd_dq_kernel: rows = queries (f0 + ...), cols = keys (s0r + ...) ----
-        const int q0 = f0, k0 = s0r;
-        uint32_t w[2][2] = {{0xffffffffu, 0xffffffffu}, {0xffffffffu, 0xffffffffu}};
-        if (flag == 1) {
-#pragma unroll
-          for (int r = 0; r < 2; ++r) {
-            const int row = q0 + wq * 16 + gr + r * 8;
-#pragma unroll
-            for (int ww = 0; ww < 2; ++ww) {
-              const int wi = t * 2 + ww;
-              w[r][ww] = (row < p.Lq && wi < p.mask_words) ? p.mask[static_cast<long long>(row) * p.mask_words + wi] : 0u;
-            }
-          }
-        }
-        if (p.drop_scale != 0.f) dropout_bits(p, bh, q0 + wq * 16, k0, false, keep);
-#pragma unroll
-        for (int tt = 0; tt < 8; ++tt) {
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const int r = e >> 1;
-            const int kk = tt * 8 + 2 * c + (e & 1);
-            bool vis = (k0 + kk < p.Lk);
-            if (flag == 1) vis = vis && ((w[r][kk >> 5] >> (kk & 31)) & 1u);
-            const float pv = vis ? exp2f(s[tt][e] * sc - lse2[r]) : 0.f;
-            float dpv = dp[tt][e];
-            if (p.drop_scale != 0.f) dpv = ((keep[tt] >> e) & 1u) ? dpv * p.drop_scale : 0.f;
-            s[tt][e] = pv * (dpv - dlt[r]);
-          }
-        }
+        // rows = queries (f0 + ...), cols = keys (s0r + ...)
+        dq_form_ds(p, sc, bh, f0 + wq * 16, s0r, flag, lse2, dlt, s, dp);
         uint32_t da[4][4];
         c_to_a(s, da);
         float (&dqd)[32] = *reinterpret_cast<float(*)[32]>(&acc0[0][0]);
@@ -945,26 +870,11 @@ __global__ void __launch_bounds__(WF_THREADS, 1) attn_bwd_wgmma_kernel(const __g
     if (++st == WF_STAGES) { st = 0; ph ^= 1; }
   }
   if (g == 1 && !has1) return;
-
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const int row = f0 + wq * 16 + gr + r * 8;
-    if (DKV) {
-      if (row < p.Lk) {
-        bf16* dkd = p.dk + b * p.dk_sb + static_cast<long long>(row) * p.dk_ss + h * p.dk_sh;
-        bf16* dvd = p.dv + b * p.dv_sb + static_cast<long long>(row) * p.dv_ss + h * p.dv_sh;
-#pragma unroll
-        for (int tt = 0; tt < 8; ++tt) {
-          *reinterpret_cast<uint32_t*>(dkd + tt * 8 + 2 * c) = pack_bf16x2(acc0[tt][2 * r] * p.scale, acc0[tt][2 * r + 1] * p.scale);
-          *reinterpret_cast<uint32_t*>(dvd + tt * 8 + 2 * c) = pack_bf16x2(acc1[tt][2 * r], acc1[tt][2 * r + 1]);
-        }
-      }
-    } else if (row < p.Lq) {
-      bf16* dst = p.dq + b * p.dq_sb + static_cast<long long>(row) * p.dq_ss + h * p.dq_sh;
-#pragma unroll
-      for (int tt = 0; tt < 8; ++tt)
-        *reinterpret_cast<uint32_t*>(dst + tt * 8 + 2 * c) = pack_bf16x2(acc0[tt][2 * r] * p.scale, acc0[tt][2 * r + 1] * p.scale);
-    }
+  if (DKV) {
+    store_frag_bf16(p.dk + b * p.dk_sb + h * p.dk_sh, p.dk_ss, f0 + wq * 16, p.Lk, acc0, p.scale);
+    store_frag_bf16(p.dv + b * p.dv_sb + h * p.dv_sh, p.dv_ss, f0 + wq * 16, p.Lk, acc1, 1.f);
+  } else {
+    store_frag_bf16(p.dq + b * p.dq_sb + h * p.dq_sh, p.dq_ss, f0 + wq * 16, p.Lq, acc0, p.scale);
   }
 }
 constexpr int WB_SMEM = 1024 + 4 * 8192 + WF_STAGES * 2 * 8192 + 128;
@@ -1081,8 +991,7 @@ static int attn_fwd_wgmma_launch(const dvla_attn_fwd_args* a, const AttnParams& 
     return DVLA_ERR_CUDA;
   static std::once_flag once;
   static cudaError_t attr_err = cudaSuccess;
-  std::call_once(once, [] { attr_err = cudaFuncSetAttribute(attn_fwd_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WF_SMEM); });
-  if (attr_err != cudaSuccess) { set_error("attn_fwd_wgmma smem attribute: %s", cudaGetErrorString(attr_err)); return DVLA_ERR_CUDA; }
+  if (!set_smem_attr_once(once, attr_err, attn_fwd_wgmma_kernel, WF_SMEM)) { set_error("attn_fwd_wgmma smem attribute: %s", cudaGetErrorString(attr_err)); return DVLA_ERR_CUDA; }
   attn_fwd_wgmma_kernel<<<dim3(p.H, p.B, (p.nqt + 1) / 2), WF_THREADS, WF_SMEM, s>>>(tm, p);
   DVLA_CHECK_LAUNCH("attn_fwd_wgmma");
   return DVLA_OK;
@@ -1092,8 +1001,7 @@ template <bool DKV>
 static int attn_bwd_wgmma_launch(const WgmmaBwdMaps& tm, const AttnParams& p, cudaStream_t s) {
   static std::once_flag once;
   static cudaError_t attr_err = cudaSuccess;
-  std::call_once(once, [] { attr_err = cudaFuncSetAttribute(attn_bwd_wgmma_kernel<DKV>, cudaFuncAttributeMaxDynamicSharedMemorySize, WB_SMEM); });
-  if (attr_err != cudaSuccess) { set_error("attn_bwd_wgmma smem attribute: %s", cudaGetErrorString(attr_err)); return DVLA_ERR_CUDA; }
+  if (!set_smem_attr_once(once, attr_err, attn_bwd_wgmma_kernel<DKV>, WB_SMEM)) { set_error("attn_bwd_wgmma smem attribute: %s", cudaGetErrorString(attr_err)); return DVLA_ERR_CUDA; }
   const int nf = DKV ? p.nkt : p.nqt;
   attn_bwd_wgmma_kernel<DKV><<<dim3(p.H, p.B, (nf + 1) / 2), WF_THREADS, WB_SMEM, s>>>(tm, p);
   DVLA_CHECK_LAUNCH(DKV ? "attn_bwd_dkv_wgmma" : "attn_bwd_dq_wgmma");
@@ -1137,15 +1045,11 @@ extern "C" int dvla_attn_fwd(const dvla_attn_fwd_args* a, void* stream) {
   if (a->mask && a->mask_words * 32 < a->Lk) { set_error("attn_fwd: mask_words too small"); return DVLA_ERR_INVALID; }
   if (a->mask && !a->tile_flags) { set_error("attn_fwd: mask given without tile_flags"); return DVLA_ERR_INVALID; }
   if (!dropout_rate_ok(a->dropout_p)) { set_error("attn_fwd: dropout_p out of range [0, 1)"); return DVLA_ERR_INVALID; }
+  if (attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p)) return attn_small_fwd(a, s);
   if (a->key_bias) {
-    if (!attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p)) {
-      set_error("attn_fwd: key_bias needs the short-sequence kernels (Lq <= 32, Lk <= 64, no mask, no dropout)");
-      return DVLA_ERR_UNSUPPORTED;
-    }
-    return attn_small_fwd(a, s);
+    set_error("attn_fwd: key_bias needs the short-sequence kernels (Lq <= 32, Lk <= 64, no mask, no dropout)");
+    return DVLA_ERR_UNSUPPORTED;
   }
-  if (attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p))
-    return attn_small_fwd(a, s);
   AttnParams p = attn_params(a);
   p.out = (bf16*)a->o;
   // wgmma + TMA for the long sequences (backbone, ViT, decoders); the mma.sync kernel for short query blocks and strides a
@@ -1172,15 +1076,11 @@ extern "C" int dvla_attn_bwd(const dvla_attn_bwd_args* a, void* stream) {
   if (a->B <= 0 || a->H <= 0 || a->Lq <= 0 || a->Lk <= 0) { set_error("attn_bwd: non-positive dims"); return DVLA_ERR_INVALID; }
   if (a->mask && !a->tile_flags) { set_error("attn_bwd: mask given without tile_flags"); return DVLA_ERR_INVALID; }
   if (!dropout_rate_ok(a->dropout_p)) { set_error("attn_bwd: dropout_p out of range [0, 1)"); return DVLA_ERR_INVALID; }
+  if (attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p)) return attn_small_bwd(a, s);   // writes delta itself
   if (a->key_bias) {
-    if (!attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p)) {
-      set_error("attn_bwd: key_bias needs the short-sequence kernels (Lq <= 32, Lk <= 64, no mask, no dropout)");
-      return DVLA_ERR_UNSUPPORTED;
-    }
-    return attn_small_bwd(a, s);
+    set_error("attn_bwd: key_bias needs the short-sequence kernels (Lq <= 32, Lk <= 64, no mask, no dropout)");
+    return DVLA_ERR_UNSUPPORTED;
   }
-  if (attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p))
-    return attn_small_bwd(a, s);          // writes delta itself
   AttnParams p = attn_params(a);
   p.o = (const bf16*)a->o; p.d_o = (const bf16*)a->d_o; p.dq = (bf16*)a->dq; p.dk = (bf16*)a->dk; p.dv = (bf16*)a->dv;
   p.delta = a->delta;

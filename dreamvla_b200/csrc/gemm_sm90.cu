@@ -692,13 +692,6 @@ bool make_tmap_2d_bf16(CUtensorMap* out, const void* base, uint64_t inner, uint6
   return true;
 }
 
-// cudaFuncSetAttribute once per kernel instantiation, race-free between the forward and the autograd thread
-template <typename K>
-static bool set_smem_attr_once(std::once_flag& once, cudaError_t& err, K kern, int bytes) {
-  std::call_once(once, [&] { err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes); });
-  return err == cudaSuccess;
-}
-
 template <bool A_MN, bool B_MN>
 static int launch_tc(const dvla_gemm_args* a, const GemmParams& p, cudaStream_t stream) {
   using Cfg = GemmCfg;

@@ -5,6 +5,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <mutex>
+
 #include "../../include/dvla.h"
 
 namespace dvla {
@@ -28,6 +30,14 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 EncodeTiledFn get_encode_fn();
+
+// cudaFuncSetAttribute once per kernel instantiation (the caller's static `once` and `err`), race-free between the
+// forward and the autograd thread; false if it failed, with the error in `err`.
+template <typename K>
+bool set_smem_attr_once(std::once_flag& once, cudaError_t& err, K kern, int bytes) {
+  std::call_once(once, [&] { err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes); });
+  return err == cudaSuccess;
+}
 
 // Dropout rates the ABI accepts: [0, 1).  Written so that NaN fails too.
 inline bool dropout_rate_ok(float p) { return p >= 0.f && p < 1.f; }
