@@ -50,7 +50,7 @@ class AttnFwdArgs(C.Structure):
                 ("q_sb", _i64), ("q_ss", _i64), ("q_sh", _i64), ("k_sb", _i64), ("k_ss", _i64), ("k_sh", _i64),
                 ("v_sb", _i64), ("v_ss", _i64), ("v_sh", _i64), ("o_sb", _i64), ("o_ss", _i64), ("o_sh", _i64),
                 ("mask_words", _i32), ("scale", _f32), ("dropout_p", _f32), ("dropout_seed", _u64), ("dropout_seed_ptr", _vp),
-                ("key_bias", _vp)]
+                ("key_bias", _vp), ("head_dim", _i64)]
 
 
 class AttnBwdArgs(C.Structure):
@@ -63,7 +63,7 @@ class AttnBwdArgs(C.Structure):
                 ("dq_sb", _i64), ("dq_ss", _i64), ("dq_sh", _i64), ("dk_sb", _i64), ("dk_ss", _i64), ("dk_sh", _i64),
                 ("dv_sb", _i64), ("dv_ss", _i64), ("dv_sh", _i64),
                 ("mask_words", _i32), ("scale", _f32), ("dropout_p", _f32), ("dropout_seed", _u64), ("dropout_seed_ptr", _vp),
-                ("mask_t", _vp), ("mask_t_words", _i32), ("key_bias", _vp)]
+                ("mask_t", _vp), ("mask_t_words", _i32), ("key_bias", _vp), ("head_dim", _i64)]
 
 
 class AdamWArgs(C.Structure):
@@ -276,28 +276,29 @@ def layernorm_bwd(dy2d, x2d, gamma, mean, rstd, dgamma_f32, dbeta_f32, dres2d=No
     return dx
 
 
-def _bsh(t):
-    """[B, L, H, 64] view -> (batch, seq, head) element strides."""
-    assert t.dim() == 4 and t.shape[-1] == 64 and t.stride(3) == 1 and t.dtype == torch.bfloat16, (t.shape, t.stride())
+def _bsh(t, hd=64):
+    """[B, L, H, hd] view -> (batch, seq, head) element strides."""
+    assert t.dim() == 4 and t.shape[-1] == hd and t.stride(3) == 1 and t.dtype == torch.bfloat16, (t.shape, t.stride())
     return t.stride(0), t.stride(1), t.stride(2)
 
 
 def attn_fwd(q, k, v, scale, mask_bits=None, tile_flags=None, dropout_p=0.0, dropout_seed=0, need_lse=True,
              dropout_seed_ptr=None, key_bias=None):
-    """q [B,Lq,H,64], k/v [B,Lk,H,64] (arbitrary batch/seq/head strides) -> o [B,Lq,H,64] contiguous, lse [B,H,Lq]."""
+    """q [B,Lq,H,hd], k/v [B,Lk,H,hd] (arbitrary batch/seq/head strides) -> o [B,Lq,H,hd] contiguous, lse [B,H,Lq].
+    hd = 64, or 96 where the short-sequence kernels run (the library refuses other cases)."""
     _need_cuda(q, k, v)
-    B, Lq, H, _ = q.shape
+    B, Lq, H, hd = q.shape
     Lk = k.shape[1]
-    o = torch.empty((B, Lq, H, 64), device=q.device, dtype=torch.bfloat16)
+    o = torch.empty((B, Lq, H, hd), device=q.device, dtype=torch.bfloat16)
     lse = torch.empty((B, H, Lq), device=q.device, dtype=torch.float32) if need_lse else None
     a = AttnFwdArgs()
     a.q, a.k, a.v, a.o, a.lse = q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), _ptr(lse)
     a.mask, a.tile_flags = _ptr(mask_bits), _ptr(tile_flags)
-    a.B, a.H, a.Lq, a.Lk = B, H, Lq, Lk
-    a.q_sb, a.q_ss, a.q_sh = _bsh(q)
-    a.k_sb, a.k_ss, a.k_sh = _bsh(k)
-    a.v_sb, a.v_ss, a.v_sh = _bsh(v)
-    a.o_sb, a.o_ss, a.o_sh = _bsh(o)
+    a.B, a.H, a.Lq, a.Lk, a.head_dim = B, H, Lq, Lk, hd
+    a.q_sb, a.q_ss, a.q_sh = _bsh(q, hd)
+    a.k_sb, a.k_ss, a.k_sh = _bsh(k, hd)
+    a.v_sb, a.v_ss, a.v_sh = _bsh(v, hd)
+    a.o_sb, a.o_ss, a.o_sh = _bsh(o, hd)
     a.mask_words = 0 if mask_bits is None else mask_bits.shape[1]
     a.scale, a.dropout_p, a.dropout_seed = float(scale), float(dropout_p), int(dropout_seed)
     a.dropout_seed_ptr = _ptr(dropout_seed_ptr)
@@ -310,7 +311,7 @@ def attn_fwd(q, k, v, scale, mask_bits=None, tile_flags=None, dropout_p=0.0, dro
 
 def attn_bwd(q, k, v, o, d_o, lse, scale, dq, dk, dv, mask_bits=None, tile_flags=None, dropout_p=0.0, dropout_seed=0,
              dropout_seed_ptr=None, key_bias=None):
-    B, Lq, H, _ = q.shape
+    B, Lq, H, hd = q.shape
     Lk = k.shape[1]
     ws = load().dvla_attn_bwd_workspace_bytes(B, H, Lq)
     delta = torch.empty(ws // 4, device=q.device, dtype=torch.float32)
@@ -319,15 +320,15 @@ def attn_bwd(q, k, v, o, d_o, lse, scale, dq, dk, dv, mask_bits=None, tile_flags
     a.lse, a.delta = lse.data_ptr(), delta.data_ptr()
     a.dq, a.dk, a.dv = dq.data_ptr(), dk.data_ptr(), dv.data_ptr()
     a.mask, a.tile_flags = _ptr(mask_bits), _ptr(tile_flags)
-    a.B, a.H, a.Lq, a.Lk = B, H, Lq, Lk
-    a.q_sb, a.q_ss, a.q_sh = _bsh(q)
-    a.k_sb, a.k_ss, a.k_sh = _bsh(k)
-    a.v_sb, a.v_ss, a.v_sh = _bsh(v)
-    a.o_sb, a.o_ss, a.o_sh = _bsh(o)
-    a.do_sb, a.do_ss, a.do_sh = _bsh(d_o)
-    a.dq_sb, a.dq_ss, a.dq_sh = _bsh(dq)
-    a.dk_sb, a.dk_ss, a.dk_sh = _bsh(dk)
-    a.dv_sb, a.dv_ss, a.dv_sh = _bsh(dv)
+    a.B, a.H, a.Lq, a.Lk, a.head_dim = B, H, Lq, Lk, hd
+    a.q_sb, a.q_ss, a.q_sh = _bsh(q, hd)
+    a.k_sb, a.k_ss, a.k_sh = _bsh(k, hd)
+    a.v_sb, a.v_ss, a.v_sh = _bsh(v, hd)
+    a.o_sb, a.o_ss, a.o_sh = _bsh(o, hd)
+    a.do_sb, a.do_ss, a.do_sh = _bsh(d_o, hd)
+    a.dq_sb, a.dq_ss, a.dq_sh = _bsh(dq, hd)
+    a.dk_sb, a.dk_ss, a.dk_sh = _bsh(dk, hd)
+    a.dv_sb, a.dv_ss, a.dv_sh = _bsh(dv, hd)
     a.mask_words = 0 if mask_bits is None else mask_bits.shape[1]
     a.scale, a.dropout_p, a.dropout_seed = float(scale), float(dropout_p), int(dropout_seed)
     a.dropout_seed_ptr = _ptr(dropout_seed_ptr)

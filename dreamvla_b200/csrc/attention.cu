@@ -1,4 +1,5 @@
-// Flash-style multi-head attention for head_dim = 64 with a bit-matrix visibility mask and tile skipping.
+// Flash-style multi-head attention for head_dim = 64 with a bit-matrix visibility mask and tile skipping.  The entry points
+// also route the short-sequence case (head_dim 64 or 96) to attention_small.cu.
 //
 // Data path of the mma.sync kernels: cp.async -> XOR-swizzled smem tiles -> ldmatrix -> mma.sync.m16n8k16 (bf16, fp32 accumulate),
 // online softmax in registers, no [Lq,Lk] tensor in HBM.  These serve short query blocks and strides a tensor map cannot
@@ -954,6 +955,16 @@ bool attn_small_applicable(int64_t Lq, int64_t Lk, const void* mask, float dropo
 int attn_small_fwd(const dvla_attn_fwd_args* a, cudaStream_t s);
 int attn_small_bwd(const dvla_attn_bwd_args* a, cudaStream_t s);
 
+// head_dim 0 (callers built before the field existed) and 64 run on every kernel; 96 only on the short-sequence ones.
+static bool head_dim_ok(int64_t head_dim, bool small) { return head_dim == 0 || head_dim == 64 || (head_dim == 96 && small); }
+template <class Args>
+static int head_dim_unsupported(const char* op, const Args* a) {
+  set_error("%s: head_dim %lld unsupported: 64, or 96 on the short-sequence kernels only (Lq <= 32, Lk <= 64, no mask, "
+            "no dropout); got Lq=%lld Lk=%lld mask=%s dropout_p=%g", op, (long long)a->head_dim, (long long)a->Lq,
+            (long long)a->Lk, a->mask ? "yes" : "no", (double)a->dropout_p);
+  return DVLA_ERR_UNSUPPORTED;
+}
+
 // [B, L, H, 64] strided view -> 4-D tensor map with 64 x 64 boxes, 128-byte swizzle (the layout the wgmma descriptors
 // expect); seq and head dims are ordered so that the strides ascend.
 static bool make_attn_tmap(CUtensorMap* out, const void* base, long long L, long long H, long long B, long long ss,
@@ -1045,7 +1056,9 @@ extern "C" int dvla_attn_fwd(const dvla_attn_fwd_args* a, void* stream) {
   if (a->mask && a->mask_words * 32 < a->Lk) { set_error("attn_fwd: mask_words too small"); return DVLA_ERR_INVALID; }
   if (a->mask && !a->tile_flags) { set_error("attn_fwd: mask given without tile_flags"); return DVLA_ERR_INVALID; }
   if (!dropout_rate_ok(a->dropout_p)) { set_error("attn_fwd: dropout_p out of range [0, 1)"); return DVLA_ERR_INVALID; }
-  if (attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p)) return attn_small_fwd(a, s);
+  const bool small = attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p);
+  if (!head_dim_ok(a->head_dim, small)) return head_dim_unsupported("attn_fwd", a);
+  if (small) return attn_small_fwd(a, s);
   if (a->key_bias) {
     set_error("attn_fwd: key_bias needs the short-sequence kernels (Lq <= 32, Lk <= 64, no mask, no dropout)");
     return DVLA_ERR_UNSUPPORTED;
@@ -1076,7 +1089,9 @@ extern "C" int dvla_attn_bwd(const dvla_attn_bwd_args* a, void* stream) {
   if (a->B <= 0 || a->H <= 0 || a->Lq <= 0 || a->Lk <= 0) { set_error("attn_bwd: non-positive dims"); return DVLA_ERR_INVALID; }
   if (a->mask && !a->tile_flags) { set_error("attn_bwd: mask given without tile_flags"); return DVLA_ERR_INVALID; }
   if (!dropout_rate_ok(a->dropout_p)) { set_error("attn_bwd: dropout_p out of range [0, 1)"); return DVLA_ERR_INVALID; }
-  if (attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p)) return attn_small_bwd(a, s);   // writes delta itself
+  const bool small = attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p);
+  if (!head_dim_ok(a->head_dim, small)) return head_dim_unsupported("attn_bwd", a);
+  if (small) return attn_small_bwd(a, s);   // writes delta itself
   if (a->key_bias) {
     set_error("attn_bwd: key_bias needs the short-sequence kernels (Lq <= 32, Lk <= 64, no mask, no dropout)");
     return DVLA_ERR_UNSUPPORTED;

@@ -4,7 +4,7 @@
 //
 // Why: at batch 1 the sampler is 10 x (12 DiT blocks + embedders + final layer + DDIM algebra) ~ 1100 kernel launches on
 // 12 token rows (2 guidance branches x 6 tokens) -- every launch is latency, none is work: the whole DiT-B is 170 MB of bf16
-// weights, i.e. ~30 us per pass at HBM speed.  Here one CTA per SM stays resident for the entire sample; every linear layer
+// weights, i.e. ~30 us per pass at HBM speed.  The same kernel runs DiT-S (head_dim 96) and DiT-L (depth 24, hidden 1024).  Here one CTA per SM stays resident for the entire sample; every linear layer
 // is a "skinny" GEMM (M <= 24 rows) in which a warp owns one output column, streams that column's weight row from HBM/L2
 // with 16-byte loads and keeps the activations (bf16) in shared memory; the phases of a block (LN+QKV | attention+proj+res |
 // LN+fc1+GELU | fc2+res) are separated by grid barriers (cooperative launch) instead of kernel boundaries.  Timestep and
@@ -247,8 +247,11 @@ __device__ __forceinline__ void stage_rows(bf16* Xs, const float* __restrict__ s
   }
 }
 
-template <int MROWS, int L>
+// HD: head_dim (64: DiT-B / DiT-L, 96: DiT-S).  In the attention phase lane l holds dims 2l, 2l+1 of a head (float2) and,
+// at HD = 96, also dim 64 + l.
+template <int MROWS, int L, int HD>
 __global__ void __launch_bounds__(DS_THREADS, 1) dit_ddim_sample_kernel(const __grid_constant__ DitSamplerParams p) {
+  static_assert(HD == 64 || HD == 96, "head_dim 64 or 96");
   extern __shared__ __align__(16) uint8_t ds_smem[];
   cg::grid_group grid = cg::this_grid();
   const int H = p.H, T = p.T, C = p.C, bs = p.bs;
@@ -319,15 +322,21 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dit_ddim_sample_kernel(const __
       // ---- P2: attention (every CTA computes all (sequence, head) pairs: 6x6 scores each) -> O in shared; h += O Wproj^T + b
       {
         bf16* Os = Xs;                                                     // [M][H] bf16
-        const float scale = 0.125f;                                       // head_dim 64
+        constexpr float scale = HD == 64 ? 0.125f : 0.10206207261596575f;    // head_dim^-0.5, as the module path's float
         for (int pr = warp; pr < nseq * p.heads; pr += DS_WARPS) {
           const int seq = pr / p.heads, hd = pr - seq * p.heads;
           float2 k[L], v[L];
-          const float* base = p.qkv + static_cast<long long>(seq * L) * 3 * H + hd * 64 + 2 * lane;
+          float k3[HD == 96 ? L : 1], v3[HD == 96 ? L : 1];           // dims 64..95 (HD = 96 only)
+          const float* base = p.qkv + static_cast<long long>(seq * L) * 3 * H + hd * HD + 2 * lane;
+          const float* base3 = base + 64 - lane;
 #pragma unroll
           for (int i = 0; i < L; ++i) {
             k[i] = __ldcg(reinterpret_cast<const float2*>(base + static_cast<long long>(i) * 3 * H + H));
             v[i] = __ldcg(reinterpret_cast<const float2*>(base + static_cast<long long>(i) * 3 * H + 2 * H));
+            if constexpr (HD == 96) {
+              k3[i] = __ldcg(base3 + static_cast<long long>(i) * 3 * H + H);
+              v3[i] = __ldcg(base3 + static_cast<long long>(i) * 3 * H + 2 * H);
+            }
           }
 #pragma unroll
           for (int i = 0; i < L; ++i) {                        // one query row at a time: L partial dots, ONE batched butterfly
@@ -335,6 +344,11 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dit_ddim_sample_kernel(const __
             float sc[L];
 #pragma unroll
             for (int j = 0; j < L; ++j) sc[j] = q.x * k[j].x + q.y * k[j].y;
+            if constexpr (HD == 96) {
+              const float q3 = __ldcg(base3 + static_cast<long long>(i) * 3 * H);
+#pragma unroll
+              for (int j = 0; j < L; ++j) sc[j] = fmaf(q3, k3[j], sc[j]);
+            }
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1)
 #pragma unroll
@@ -342,14 +356,16 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dit_ddim_sample_kernel(const __
             float mx = -INFINITY;
 #pragma unroll
             for (int j = 0; j < L; ++j) mx = fmaxf(mx, sc[j]);
-            float den = 0.f, o0 = 0.f, o1 = 0.f;
+            float den = 0.f, o0 = 0.f, o1 = 0.f, o2 = 0.f;
 #pragma unroll
             for (int j = 0; j < L; ++j) {
               const float e = __expf((sc[j] - mx) * scale);
               den += e; o0 = fmaf(e, v[j].x, o0); o1 = fmaf(e, v[j].y, o1);
+              if constexpr (HD == 96) o2 = fmaf(e, v3[j], o2);
             }
             const float inv = 1.0f / den;
-            *reinterpret_cast<uint32_t*>(Os + (seq * L + i) * H + hd * 64 + 2 * lane) = pack_bf16x2(o0 * inv, o1 * inv);
+            *reinterpret_cast<uint32_t*>(Os + (seq * L + i) * H + hd * HD + 2 * lane) = pack_bf16x2(o0 * inv, o1 * inv);
+            if constexpr (HD == 96) Os[(seq * L + i) * H + hd * HD + 64 + lane] = __float2bfloat16(o2 * inv);
           }
         }
         __syncthreads();
@@ -412,9 +428,11 @@ extern "C" int dvla_dit_ddim_sample(const dvla_dit_sampler_args* a, void* stream
   if (!a || !a->blocks || !a->z || !a->noise || !a->out || !a->workspace) { set_error("dit_ddim_sample: null pointer"); return DVLA_ERR_INVALID; }
   const int H = (int)a->hidden, T = (int)a->T, C = (int)a->channels, bs = (int)a->batch;
   const int M = 2 * bs * 2 * T;
+  const int64_t head_dim = a->heads > 0 && a->hidden % a->heads == 0 ? a->hidden / a->heads : 0;
   if (a->depth <= 0 || a->depth > DS_MAX_DEPTH || a->n_steps <= 0 || a->n_steps > DS_MAX_STEPS || M > DS_MAXM || 2 * T > 8 ||
-      a->heads * 64 != H || H % 8 || a->token % 8 || a->mlp % 8 || a->freq % 8 || bs * T + 1 > DS_MAXM) {
-    set_error("dit_ddim_sample: unsupported shape (rows %d <= %d, tokens per sequence <= 8, head_dim 64, dims %% 8)", M, DS_MAXM);
+      (head_dim != 64 && head_dim != 96) || H % 8 || a->token % 8 || a->mlp % 8 || a->freq % 8 || bs * T + 1 > DS_MAXM) {
+    set_error("dit_ddim_sample: unsupported shape (rows %d <= %d, tokens per sequence <= 8, head_dim = hidden / heads 64 or 96 "
+              "(hidden %lld, heads %lld), dims %% 8)", M, DS_MAXM, (long long)a->hidden, (long long)a->heads);
     return DVLA_ERR_UNSUPPORTED;
   }
   if (dvla_dit_sampler_workspace_bytes(a->batch, a->T, a->hidden, a->mlp, a->n_steps) > a->workspace_bytes) {
@@ -459,8 +477,11 @@ extern "C" int dvla_dit_ddim_sample(const dvla_dit_sampler_args* a, void* stream
   }
   if (smem > 227 * 1024) { set_error("dit_ddim_sample: %zu bytes of shared memory needed", smem); return DVLA_ERR_UNSUPPORTED; }
   if (2 * T != 6) { set_error("dit_ddim_sample: built for action_pred_steps == 3 (6 tokens per sequence), got %d", 2 * T); return DVLA_ERR_UNSUPPORTED; }
-  void* kern = reinterpret_cast<void*>(dit_ddim_sample_kernel<12, 6>);
-  static const cudaError_t attr_err = cudaFuncSetAttribute(dit_ddim_sample_kernel<12, 6>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+  void* kern = head_dim == 96 ? reinterpret_cast<void*>(dit_ddim_sample_kernel<12, 6, 96>)
+                              : reinterpret_cast<void*>(dit_ddim_sample_kernel<12, 6, 64>);
+  static const cudaError_t attr_err64 = cudaFuncSetAttribute(dit_ddim_sample_kernel<12, 6, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+  static const cudaError_t attr_err96 = cudaFuncSetAttribute(dit_ddim_sample_kernel<12, 6, 96>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+  const cudaError_t attr_err = head_dim == 96 ? attr_err96 : attr_err64;
   if (attr_err != cudaSuccess) { set_error("dit_ddim_sample smem attr: %s", cudaGetErrorString(attr_err)); return DVLA_ERR_CUDA; }
   if (a->n_steps > 12 || bs * T + 1 > 12) { set_error("dit_ddim_sample: prologue rows exceed 12"); return DVLA_ERR_UNSUPPORTED; }
   int dev = 0, coop = 0;

@@ -10,7 +10,7 @@ from .models import DiT
 
 
 def DiT_S(**kwargs):
-    return DiT(depth=6, hidden_size=384, num_heads=4, **kwargs)   # head_dim 96: unsupported by the attention kernels
+    return DiT(depth=6, hidden_size=384, num_heads=4, **kwargs)
 
 
 def DiT_B(**kwargs):

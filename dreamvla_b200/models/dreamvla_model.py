@@ -562,7 +562,8 @@ class DreamVLA(nn.Module):
             self.action_model.create_ddim(ddim_step=10)
         net = self.action_model.net
         if (self.FUSED_SAMPLER and 4 * bs * self.action_pred_steps <= 12 and self.action_pred_steps == 3
-                and net.x_embedder.linear.weight.shape[0] == 64 * net.num_heads and not torch.is_grad_enabled()):
+                and net.x_embedder.linear.weight.shape[0] in (64 * net.num_heads, 96 * net.num_heads)
+                and not torch.is_grad_enabled()):
             # one sequence (rollouts): the whole guided DDIM loop as one persistent kernel (csrc/dit_sampler.cu)
             from .. import _lib as L
             return L.dit_ddim_sample(net, self.action_model.ddim_diffusion, feat.to(torch.bfloat16), noise[:bs].float(),

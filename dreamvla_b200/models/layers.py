@@ -58,11 +58,12 @@ class LayerNorm(nn.LayerNorm):
 
 
 class Attention(nn.Module):
-    """timm Attention (fused qkv Linear, SDPA, proj); head_dim must be 64."""
+    """timm Attention (fused qkv Linear, SDPA, proj); head_dim 64, or 96 on short sequences (the DiT-S action head)."""
 
     def __init__(self, dim, num_heads=8, qkv_bias=False):
         super().__init__()
-        assert dim % num_heads == 0 and dim // num_heads == 64, "dreamvla_b200 attention kernels need head_dim == 64"
+        assert dim % num_heads == 0 and dim // num_heads in (64, 96), \
+            "dreamvla_b200 attention kernels need head_dim 64, or 96 on short sequences (Lq <= 32, Lk <= 64)"
         self.num_heads = num_heads
         self.head_dim = dim // num_heads
         self.scale = self.head_dim ** -0.5

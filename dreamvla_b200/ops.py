@@ -401,7 +401,7 @@ class _Attention(torch.autograd.Function):
         q, k, v, o, lse = ctx.saved_tensors
         scale, mask, dropout_p, seed, key_bias = ctx.meta
         d_o = _bf16c(d_o)
-        # if q, k, v are slices of one fused [B, L, 3, H, 64] buffer, produce the gradient in the same fused layout
+        # if q, k, v are slices of one fused [B, L, 3, H, hd] buffer, produce the gradient in the same fused layout
         fused = (q.dim() == 4 and q._base is not None and q._base is k._base and q._base is v._base and
                  q._base.dim() == 5 and q._base.shape[2] == 3 and q._base.is_contiguous())
         if fused:
@@ -419,13 +419,14 @@ class _Attention(torch.autograd.Function):
 
 
 def attention(q, k, v, scale, mask: AttnMask | None = None, dropout_p: float = 0.0, key_bias=None):
-    """q [B,Lq,H,64], k/v [B,Lk,H,64] (strided views allowed) -> [B,Lq,H,64] contiguous.
+    """q [B,Lq,H,hd], k/v [B,Lk,H,hd] (strided views allowed) -> [B,Lq,H,hd] contiguous.  hd = 64, or 96 on short
+    sequences (Lq <= 32, Lk <= 64, no mask, no dropout).
     key_bias: optional fp32 [Lk] added to the scaled scores (log r = key counted r times); short sequences only."""
     return _apply(_Attention, q, k, v, float(scale), mask, float(dropout_p), key_bias)
 
 
 class _FusedQKVAttention(torch.autograd.Function):
-    """Self-attention on a fused qkv buffer [B, L, 3, H, 64]; the backward writes one fused dqkv buffer (no cat)."""
+    """Self-attention on a fused qkv buffer [B, L, 3, H, hd]; the backward writes one fused dqkv buffer (no cat)."""
 
     @staticmethod
     def forward(ctx, qkv, scale, mask, dropout_p):
@@ -453,8 +454,8 @@ class _FusedQKVAttention(torch.autograd.Function):
 
 
 def self_attention_fused(qkv, scale, mask: AttnMask | None = None, dropout_p: float = 0.0):
-    """qkv [B, L, 3, H, 64] contiguous bf16 -> [B, L, H, 64]."""
-    assert qkv.dim() == 5 and qkv.shape[2] == 3 and qkv.shape[4] == 64 and qkv.is_contiguous()
+    """qkv [B, L, 3, H, hd] contiguous bf16 -> [B, L, H, hd]; hd = 64, or 96 on short sequences (see `attention`)."""
+    assert qkv.dim() == 5 and qkv.shape[2] == 3 and qkv.shape[4] in (64, 96) and qkv.is_contiguous()
     return _apply(_FusedQKVAttention, qkv, float(scale), mask, float(dropout_p))
 
 

@@ -124,7 +124,7 @@ typedef struct {
 int dvla_layernorm_bwd(const dvla_layernorm_bwd_args* args, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
- * Multi-head attention, head_dim = 64, flash-style (no [Lq,Lk] score tensor in HBM).
+ * Multi-head attention, head_dim = 64 (96 on the short-sequence kernels), flash-style (no [Lq,Lk] score tensor in HBM).
  *   O[b,i,h,:] = softmax_j( scale * Q[b,i,h,:].K[b,j,h,:] + maskbias(i,j) ) V[b,j,h,:]
  * Q/K/V/O are addressed with element strides (batch, seq, head) so they can alias slices of a fused QKV buffer.
  * mask: NULL (all visible) or a bit matrix [Lq, mask_words] of uint32 (bit j%32 of word j/32 set = pair (i,j) visible),
@@ -132,6 +132,9 @@ int dvla_layernorm_bwd(const dvla_layernorm_bwd_args* args, void* stream);
  * tile_flags: per (q-tile of 64, k-tile of 64) byte, 0 = skip, 1 = partial (consult bits), 2 = full; built by
  *       dvla_attn_mask_tiles from the bit matrix (NULL = all full).
  * lse: fp32 [B, H, Lq] log-sum-exp (natural log, of the scaled logits) saved for the backward, or NULL.
+ * head_dim (last field, appended after version 100 shipped; 0 means 64, so zero-initialised structs keep their meaning):
+ *       64 everywhere; 96 only where the short-sequence kernels run (Lq <= 32, Lk <= 64, no mask, no dropout; key_bias
+ *       allowed) -- the DiT-S action head.  Anything else returns DVLA_ERR_UNSUPPORTED before any launch.
  * Replaces F.scaled_dot_product_attention (timm Attention; gpt2.py:266-273), eager _attn (gpt2.py:61-84) and the
  * einsum/softmax in PerceiverAttention (perceiver_resampler.py:55-59).
  * ------------------------------------------------------------------------------------------------------------- */
@@ -154,6 +157,7 @@ typedef struct {
                                  log(r) makes key j count r times -- the identical-mask-token form of a world decoder
                                  (dreamvla_model.py:803-806 with an all-zero position embedding).  Short-sequence kernels only
                                  (Lq <= 32, Lk <= 64, no mask, no dropout); DVLA_ERR_UNSUPPORTED otherwise. */
+  int64_t head_dim;           /* 0 or 64, or 96 on the short-sequence kernels (see above) */
 } dvla_attn_fwd_args;
 int dvla_attn_fwd(const dvla_attn_fwd_args* args, void* stream);
 
@@ -175,6 +179,7 @@ typedef struct {
                                  visible); accepted for ABI compatibility, not read by the sm_90 kernels */
   int32_t mask_t_words;
   const float* key_bias;      /* as in dvla_attn_fwd_args (a constant: receives no gradient) */
+  int64_t head_dim;           /* as in dvla_attn_fwd_args */
 } dvla_attn_bwd_args;
 int dvla_attn_bwd(const dvla_attn_bwd_args* args, void* stream);
 
@@ -277,6 +282,7 @@ int dvla_grad_clip_scale(void* g_bf16, int64_t n, const float* sumsq, float max_
  * Fused action sampler: the DDIM loop of the DiT action head with classifier-free guidance as ONE persistent cooperative
  * kernel (replaces dreamvla_model.py:935-987 -> gaussian_diffusion.py:609-689 -> models.py:253-268 for small batches:
  * rows = 2 * batch * 2T <= 24).  Every pointer is device memory, weights are bf16 nn.Linear layouts [out, in].
+ * head_dim = hidden / heads must be 64 (DiT-B, DiT-L) or 96 (DiT-S); DVLA_ERR_UNSUPPORTED otherwise.
  * Schedule tables are HOST arrays of n_steps entries (respaced DDIM: timestep_map[i] is the original timestep of step i).
  * ------------------------------------------------------------------------------------------------------------- */
 typedef struct {
