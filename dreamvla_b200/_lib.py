@@ -94,7 +94,11 @@ class DitSamplerArgs(C.Structure):
                                    "final_b", "z", "noise", "out")] + \
                [("timestep_map", C.POINTER(_i32)), ("sqrt_recip_alphas_cumprod", C.POINTER(_f32)),
                 ("sqrt_recipm1_alphas_cumprod", C.POINTER(_f32)), ("alphas_cumprod_prev", C.POINTER(_f32)),
-                ("n_steps", _i64), ("cfg_scale", _f32), ("workspace", _vp), ("workspace_bytes", _i64)]
+                ("n_steps", _i64), ("cfg_scale", _f32), ("workspace", _vp), ("workspace_bytes", _i64),
+                ("integrator", _i64), ("t_values", C.POINTER(_f32))]
+
+
+DIT_DDIM, DIT_FM_EULER = 0, 1     # dvla_dit_sampler_args.integrator
 
 
 # name -> (restype, argtypes) of every function include/dvla.h declares; tests/test_abi_cpu.py checks it against the header.
@@ -541,15 +545,14 @@ def cat_broadcast(e, m):
     return out
 
 
-def dit_ddim_sample(net, diffusion, z, noise, cfg_scale):
-    """Fused DDIM sampler of the DiT action head (dit_sampler.cu): z bf16 [bs, T, token] condition rows, noise fp32 [bs, T, C]
-    -> fp32 [bs, T, C].  `net` is models.action_model.models.DiT, `diffusion` the respaced SpacedDiffusion."""
+def _dit_sampler_call(net, z, noise, n_steps, cfg_scale, fill):
+    """Sets up dvla_dit_sampler_args for `net` (models.action_model.models.DiT) on condition rows z bf16 [bs, T, token] and the
+    start state noise fp32 [bs, T, C], lets `fill(args)` set the integrator's fields, launches; -> fp32 [bs, T, C]."""
     _need_cuda(z, noise)
     bs, T, token = z.shape
     Cc = noise.shape[-1]
     H = net.x_embedder.linear.weight.shape[0]
     mlp = net.blocks[0].mlp.fc1.weight.shape[0]
-    n_steps = diffusion.num_timesteps
     blocks = (DitBlockWeights * len(net.blocks))()
     for i, b in enumerate(net.blocks):
         blocks[i] = DitBlockWeights(b.attn.qkv.weight.data_ptr(), b.attn.qkv.bias.data_ptr(), b.attn.proj.weight.data_ptr(),
@@ -560,8 +563,6 @@ def dit_ddim_sample(net, diffusion, z, noise, cfg_scale):
     out = torch.empty((bs, T, Cc), device=z.device, dtype=torch.float32)
     ws_bytes = load().dvla_dit_sampler_workspace_bytes(bs, T, H, mlp, n_steps)
     ws = torch.empty(ws_bytes, device=z.device, dtype=torch.uint8)
-    tmap = (_i32 * n_steps)(*[int(t) for t in diffusion.timestep_map])
-    f32arr = lambda a: (_f32 * n_steps)(*[float(v) for v in a])     # noqa: E731
     a = DitSamplerArgs()
     a.blocks = blocks
     a.depth, a.hidden, a.heads, a.mlp, a.token = len(net.blocks), H, net.num_heads, mlp, token
@@ -573,11 +574,44 @@ def dit_ddim_sample(net, diffusion, z, noise, cfg_scale):
     a.uncondition, a.pos = net.z_embedder.uncondition.data_ptr(), net.positional_embedding.data_ptr()
     a.final_w, a.final_b = net.final_layer.linear.weight.data_ptr(), net.final_layer.linear.bias.data_ptr()
     a.z, a.noise, a.out = z.data_ptr(), noise.data_ptr(), out.data_ptr()
-    a.timestep_map = tmap
-    a.sqrt_recip_alphas_cumprod = f32arr(diffusion.sqrt_recip_alphas_cumprod)
-    a.sqrt_recipm1_alphas_cumprod = f32arr(diffusion.sqrt_recipm1_alphas_cumprod)
-    a.alphas_cumprod_prev = f32arr(diffusion.alphas_cumprod_prev)
     a.n_steps, a.cfg_scale = n_steps, float(cfg_scale)
     a.workspace, a.workspace_bytes = ws.data_ptr(), ws_bytes
+    fill(a)
     _call("dvla_dit_ddim_sample", C.byref(a), _stream())
     return out
+
+
+def dit_ddim_sample(net, diffusion, z, noise, cfg_scale):
+    """Fused DDIM sampler of the DiT action head (dit_sampler.cu): z bf16 [bs, T, token] condition rows, noise fp32 [bs, T, C]
+    -> fp32 [bs, T, C].  `net` is models.action_model.models.DiT, `diffusion` the respaced SpacedDiffusion."""
+    n_steps = diffusion.num_timesteps
+
+    def fill(a):
+        f32arr = lambda v: (_f32 * n_steps)(*[float(x) for x in v])     # noqa: E731
+        a.timestep_map = (_i32 * n_steps)(*[int(t) for t in diffusion.timestep_map])
+        a.sqrt_recip_alphas_cumprod = f32arr(diffusion.sqrt_recip_alphas_cumprod)
+        a.sqrt_recipm1_alphas_cumprod = f32arr(diffusion.sqrt_recipm1_alphas_cumprod)
+        a.alphas_cumprod_prev = f32arr(diffusion.alphas_cumprod_prev)
+        a.integrator = DIT_DDIM
+    return _dit_sampler_call(net, z, noise, n_steps, cfg_scale, fill)
+
+
+def fm_t_values(n_steps):
+    """The DiT timestep input of each flow-matching step, in execution order: fp32 i / n_steps, i = 0 .. n_steps-1, divided
+    in fp32 as FMDiffusion.ddim_sample_loop's `torch.full((n,), float(i)) / T` (gaussian_diffusion.py:169) divides.  (On a
+    CUDA tensor torch computes that division as a multiply by the fp32 reciprocal, one ulp off at i = 9 of 10: 0.90000004
+    against 0.89999998 -- far below the bf16 rounding of the frequency features the value feeds.)"""
+    return [float(v) for v in torch.arange(n_steps, dtype=torch.float32) / n_steps]
+
+
+def dit_fm_sample(net, diffusion, z, start):
+    """Fused flow-matching sampler of the DiT action head (`--use_fm`; dit_sampler.cu with the Euler integrator): z bf16
+    [bs, T, token] condition rows, start fp32 [bs, T, C] start state -> fp32 [bs, T, C], as FMDiffusion.ddim_sample_loop
+    (`diffusion`) computes the first half of its [2 bs, ...] state: guidance scale 1.0 over both branches, num_timesteps Euler
+    steps of 1 / num_timesteps."""
+    n_steps = diffusion.num_timesteps
+
+    def fill(a):
+        a.t_values = (_f32 * n_steps)(*fm_t_values(n_steps))
+        a.integrator = DIT_FM_EULER
+    return _dit_sampler_call(net, z, start, n_steps, 1.0, fill)

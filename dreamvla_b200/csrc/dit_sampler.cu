@@ -1,6 +1,7 @@
 // Whole-sampler kernel for action inference: the 10-step DDIM loop of the DiT action head with classifier-free guidance
 // (reference models/dreamvla_model.py:935-987 -> action_model.py:76-83 -> gaussian_diffusion.py:522-569,609-689 ->
-// models.py:234-268) as ONE persistent cooperative kernel.
+// models.py:234-268) as ONE persistent cooperative kernel.  The flow-matching head (`--use_fm`, respace.py:118-191) runs the
+// same kernel with an Euler integrator in place of the DDIM update (template parameter INTEG, see below).
 //
 // Why: at batch 1 the sampler is 10 x (12 DiT blocks + embedders + final layer + DDIM algebra) ~ 1100 kernel launches on
 // 12 token rows (2 guidance branches x 6 tokens) -- every launch is latency, none is work: the whole DiT-B is 170 MB of bf16
@@ -48,6 +49,9 @@ struct DitSamplerParams {
   float cfg_scale;
   int bs, T, C, H, heads, token, mlp, freq;
   float *h0, *h1, *qkv, *u, *te, *t1, *ze;     // fp32 scratch (global, L2 resident)
+  // flow matching only (behind the DDIM fields, whose parameter offsets -- and so the DDIM code -- stay as they were)
+  float tval[DS_MAX_STEPS];  // DiT timestep input of step i, in execution order
+  float fm_delta;            // Euler step 1 / n_steps
 };
 
 __device__ __forceinline__ float warp_sum_f(float v) {
@@ -249,9 +253,18 @@ __device__ __forceinline__ void stage_rows(bf16* Xs, const float* __restrict__ s
 
 // HD: head_dim (64: DiT-B / DiT-L, 96: DiT-S).  In the attention phase lane l holds dims 2l, 2l+1 of a head (float2) and,
 // at HD = 96, also dim 64 + l.
-template <int MROWS, int L, int HD>
+// INTEG: the integrator (include/dvla.h `integrator`).
+//   DS_DDIM: steps n-1 .. 0, timestep input timestep_map[step], start state bf16(noise), eta = 0 DDIM update.
+//   DS_FM:   flow-matching Euler as FMDiffusion.ddim_sample_loop (gaussian_diffusion.py:158-172): steps 0 .. n-1, timestep input
+//            the fp32 t_values[step] (= step / n), start state the fp32 noise as given (x is rounded to bf16 only where it enters
+//            x_embedder, as in the module path), update x += bf16(delta * u) with u the bf16 guided output (`final + delta * ut`
+//            on a bf16 ut).
+enum { DS_DDIM = 0, DS_FM = 1 };
+template <int MROWS, int L, int HD, int INTEG>
 __global__ void __launch_bounds__(DS_THREADS, 1) dit_ddim_sample_kernel(const __grid_constant__ DitSamplerParams p) {
   static_assert(HD == 64 || HD == 96, "head_dim 64 or 96");
+  static_assert(INTEG == DS_DDIM || INTEG == DS_FM, "integrator");
+  constexpr bool FM = INTEG == DS_FM;
   extern __shared__ __align__(16) uint8_t ds_smem[];
   cg::grid_group grid = cg::this_grid();
   const int H = p.H, T = p.T, C = p.C, bs = p.bs;
@@ -269,7 +282,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dit_ddim_sample_kernel(const __
   for (int i = tid; i < p.n_steps * p.freq; i += DS_THREADS) {
     const int s = i / p.freq, k = i - s * p.freq, half = p.freq >> 1;
     const float fr = __expf(-9.210340371976184f * static_cast<float>(k < half ? k : k - half) / half);   // ln(10000)
-    const float a = static_cast<float>(p.tmap[s]) * fr;
+    const float a = (FM ? p.tval[s] : static_cast<float>(p.tmap[s])) * fr;
     Xs[i] = __float2bfloat16(k < half ? cosf(a) : sinf(a));
   }
   __syncthreads();
@@ -284,7 +297,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dit_ddim_sample_kernel(const __
     __syncthreads();
     skinny_gemm<MROWS>(Xs, rows, p.token, p.z_w, p.z_b, H, p.ze, H, EPI_STORE);
   }
-  for (int i = tid; i < bs * T * C; i += DS_THREADS) xcur[i] = __bfloat162float(__float2bfloat16(p.noise[i]));
+  for (int i = tid; i < bs * T * C; i += DS_THREADS) xcur[i] = FM ? p.noise[i] : __bfloat162float(__float2bfloat16(p.noise[i]));
   grid.sync();
   // ---- prologue B: te = W2 t1 + b2
   stage_rows(Xs, p.t1, p.n_steps * H);
@@ -292,7 +305,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dit_ddim_sample_kernel(const __
   skinny_gemm<MROWS>(Xs, p.n_steps, H, p.t2_w, p.t2_b, H, p.te, H, EPI_STORE);
   grid.sync();
 
-  for (int step = p.n_steps - 1, it = 0; step >= 0; --step, ++it) {
+  for (int step = FM ? 0 : p.n_steps - 1, it = 0; FM ? step < p.n_steps : step >= 0; step += FM ? 1 : -1, ++it) {
     float* h = (it & 1) ? p.h1 : p.h0;
     // ---- H0: token rows.  row = seq * L + tok; tok < T: te + ze (+ pos); tok >= T: x_embedder(x) (+ pos)
     for (int i = gtid; i < M * H; i += gthreads) {
@@ -383,7 +396,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dit_ddim_sample_kernel(const __
       skinny_gemm<MROWS>(Xs, M, p.mlp, w.fc2_w, w.fc2_b, H, h, H, EPI_ACC);
       grid.sync();
     }
-    // ---- final layer on the action rows + guidance + DDIM update: redundantly in every CTA (x stays in shared memory).
+    // ---- final layer on the action rows + guidance + DDIM / Euler update: redundantly in every CTA (x stays in shared memory).
     //      h of this step is not written again before two more grid barriers (the next step uses the other h buffer).
     {
       const int arows = nseq * T;
@@ -405,16 +418,29 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dit_ddim_sample_kernel(const __
         const float cond = eps_s[b * T * C + rem], unc = eps_s[(bs + b) * T * C + rem];
         const float eps = __bfloat162float(__float2bfloat16(unc + p.cfg_scale * (cond - unc)));     // models.py:262-266
         const float x = xcur[i];
-        const float x0 = p.sqrt_recip[step] * x - p.sqrt_recipm1[step] * eps;                       // gaussian_diffusion.py:328,345
-        const float e2 = (p.sqrt_recip[step] * x - x0) / p.sqrt_recipm1[step];                      // :554
-        const float ab = p.acp_prev[step];
-        xcur[i] = x0 * sqrtf(ab) + sqrtf(1.0f - ab) * e2;                                            // :560-565, eta = 0
+        if constexpr (FM) {
+          xcur[i] = x + __bfloat162float(__float2bfloat16(p.fm_delta * eps));                        // gaussian_diffusion.py:171
+        } else {
+          const float x0 = p.sqrt_recip[step] * x - p.sqrt_recipm1[step] * eps;                     // gaussian_diffusion.py:328,345
+          const float e2 = (p.sqrt_recip[step] * x - x0) / p.sqrt_recipm1[step];                    // :554
+          const float ab = p.acp_prev[step];
+          xcur[i] = x0 * sqrtf(ab) + sqrtf(1.0f - ab) * e2;                                          // :560-565, eta = 0
+        }
       }
       __syncthreads();
     }
   }
   if (blockIdx.x == 0)
     for (int i = tid; i < bs * T * C; i += DS_THREADS) p.out[i] = xcur[i];
+}
+
+// The instantiation the host launches; the shared-memory opt-in is made once per instantiation.
+template <int HD, int INTEG>
+void* sampler_kernel(cudaError_t* attr_err) {
+  static const cudaError_t e =
+      cudaFuncSetAttribute(dit_ddim_sample_kernel<12, 6, HD, INTEG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+  *attr_err = e;
+  return reinterpret_cast<void*>(dit_ddim_sample_kernel<12, 6, HD, INTEG>);
 }
 
 }  // namespace
@@ -426,6 +452,15 @@ using namespace dvla;
 extern "C" int dvla_dit_ddim_sample(const dvla_dit_sampler_args* a, void* stream) {
   const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (!a || !a->blocks || !a->z || !a->noise || !a->out || !a->workspace) { set_error("dit_ddim_sample: null pointer"); return DVLA_ERR_INVALID; }
+  if (a->integrator != DVLA_DIT_DDIM && a->integrator != DVLA_DIT_FM_EULER) {
+    set_error("dit_ddim_sample: integrator %lld unsupported (0 DDIM, 1 flow-matching Euler)", (long long)a->integrator);
+    return DVLA_ERR_UNSUPPORTED;
+  }
+  const bool fm = a->integrator == DVLA_DIT_FM_EULER;
+  if (fm && !a->t_values) { set_error("dit_ddim_sample: flow-matching Euler needs t_values (HOST [n_steps]), got NULL"); return DVLA_ERR_INVALID; }
+  if (a->n_steps > DS_MAXM) {
+    set_error("dit_ddim_sample: n_steps %lld above the %d prologue rows", (long long)a->n_steps, DS_MAXM); return DVLA_ERR_UNSUPPORTED;
+  }
   const int H = (int)a->hidden, T = (int)a->T, C = (int)a->channels, bs = (int)a->batch;
   const int M = 2 * bs * 2 * T;
   const int64_t head_dim = a->heads > 0 && a->hidden % a->heads == 0 ? a->hidden / a->heads : 0;
@@ -451,9 +486,11 @@ extern "C" int dvla_dit_ddim_sample(const dvla_dit_sampler_args* a, void* stream
   p.uncond = (const bf16*)a->uncondition; p.pos = (const bf16*)a->pos; p.fin_w = (const bf16*)a->final_w; p.fin_b = (const bf16*)a->final_b;
   p.z = (const bf16*)a->z; p.noise = a->noise; p.out = a->out;
   for (int i = 0; i < a->n_steps; ++i) {
+    if (fm) { p.tval[i] = a->t_values[i]; continue; }
     p.tmap[i] = a->timestep_map[i]; p.sqrt_recip[i] = a->sqrt_recip_alphas_cumprod[i];
     p.sqrt_recipm1[i] = a->sqrt_recipm1_alphas_cumprod[i]; p.acp_prev[i] = a->alphas_cumprod_prev[i];
   }
+  p.fm_delta = static_cast<float>(1.0 / static_cast<double>(a->n_steps));     // FMDiffusion: delta = 1.0 / T (a double), fp32 on use
   p.n_steps = (int)a->n_steps; p.cfg_scale = a->cfg_scale;
   p.bs = bs; p.T = T; p.C = C; p.H = H; p.heads = (int)a->heads; p.token = (int)a->token; p.mlp = (int)a->mlp; p.freq = (int)a->freq;
   float* ws = reinterpret_cast<float*>(a->workspace);
@@ -477,13 +514,10 @@ extern "C" int dvla_dit_ddim_sample(const dvla_dit_sampler_args* a, void* stream
   }
   if (smem > 227 * 1024) { set_error("dit_ddim_sample: %zu bytes of shared memory needed", smem); return DVLA_ERR_UNSUPPORTED; }
   if (2 * T != 6) { set_error("dit_ddim_sample: built for action_pred_steps == 3 (6 tokens per sequence), got %d", 2 * T); return DVLA_ERR_UNSUPPORTED; }
-  void* kern = head_dim == 96 ? reinterpret_cast<void*>(dit_ddim_sample_kernel<12, 6, 96>)
-                              : reinterpret_cast<void*>(dit_ddim_sample_kernel<12, 6, 64>);
-  static const cudaError_t attr_err64 = cudaFuncSetAttribute(dit_ddim_sample_kernel<12, 6, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  static const cudaError_t attr_err96 = cudaFuncSetAttribute(dit_ddim_sample_kernel<12, 6, 96>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  const cudaError_t attr_err = head_dim == 96 ? attr_err96 : attr_err64;
+  cudaError_t attr_err;
+  void* kern = head_dim == 96 ? (fm ? sampler_kernel<96, DS_FM>(&attr_err) : sampler_kernel<96, DS_DDIM>(&attr_err))
+                              : (fm ? sampler_kernel<64, DS_FM>(&attr_err) : sampler_kernel<64, DS_DDIM>(&attr_err));
   if (attr_err != cudaSuccess) { set_error("dit_ddim_sample smem attr: %s", cudaGetErrorString(attr_err)); return DVLA_ERR_CUDA; }
-  if (a->n_steps > 12 || bs * T + 1 > 12) { set_error("dit_ddim_sample: prologue rows exceed 12"); return DVLA_ERR_UNSUPPORTED; }
   int dev = 0, coop = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);

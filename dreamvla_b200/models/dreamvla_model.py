@@ -532,6 +532,14 @@ class DreamVLA(nn.Module):
 
     FUSED_SAMPLER = True
 
+    def _fused_sampler_fits(self, bs):
+        """One sequence (rollouts: 12 rows), 3 action steps, head_dim 64 or 96, no autograd: the whole guided sampler loop runs
+        as one persistent kernel (csrc/dit_sampler.cu)."""
+        net = self.action_model.net
+        return (self.FUSED_SAMPLER and 4 * bs * self.action_pred_steps <= 12 and self.action_pred_steps == 3
+                and net.x_embedder.linear.weight.shape[0] in (64 * net.num_heads, 96 * net.num_heads)
+                and not torch.is_grad_enabled())
+
     def _ddim_actions(self, feat, sample_noise, dev):
         """10-step DDIM with classifier-free guidance 1.5 (:935-987) on feat [n, action_pred_steps, D] -> [n, steps, 7]."""
         bs = feat.shape[0]
@@ -540,14 +548,21 @@ class DreamVLA(nn.Module):
             # --use_fm (ActionModelFM / FMDiffusion, respace.py:118-191): the sampler forces the guidance scale to 1.0, ignores
             # the noise it is handed and draws its own start state [2 bs, steps, 7]; `sample_noise` (parity tests) injects
             # that state ([2 bs, ...], or [bs, ...] used for both halves -- only the first half reaches the output)
-            uncondition = self.action_model.net.z_embedder.uncondition.unsqueeze(0).expand(bs, self.action_pred_steps, -1)
-            z = torch.cat([feat, uncondition], 0)
             if self.action_model.ddim_diffusion is None:
                 self.action_model.create_ddim(ddim_step=10)
+            shape = (2 * bs, self.action_pred_steps, self.action_model.in_channels)
+            if self._fused_sampler_fits(bs) and self.action_model.ddim_diffusion.num_timesteps <= 12:
+                # the same start-state draw as FMDiffusion (the CUDA generator advances alike on both paths); the kernel
+                # integrates the first half, the only one that reaches the output
+                start = sample_noise if sample_noise is not None else torch.randn(*shape, device=dev)
+                from .. import _lib as L
+                return L.dit_fm_sample(self.action_model.net, self.action_model.ddim_diffusion, feat.to(torch.bfloat16),
+                                       start[:bs].to(device=dev, dtype=torch.float32)).to(feat.dtype)
+            uncondition = self.action_model.net.z_embedder.uncondition.unsqueeze(0).expand(bs, self.action_pred_steps, -1)
+            z = torch.cat([feat, uncondition], 0)
             start = None
             if sample_noise is not None:
                 start = sample_noise if sample_noise.shape[0] == 2 * bs else torch.cat([sample_noise, sample_noise], 0)
-            shape = (2 * bs, self.action_pred_steps, self.action_model.in_channels)
             samples = self.action_model.ddim_diffusion.ddim_sample_loop(
                 self.action_model.net.forward_with_cfg, shape, None, clip_denoised=False,
                 model_kwargs=dict(z=z, cfg_scale=cfg_scale), device=dev, eta=0.0, start=start)
@@ -561,9 +576,7 @@ class DreamVLA(nn.Module):
         if self.action_model.ddim_diffusion is None:
             self.action_model.create_ddim(ddim_step=10)
         net = self.action_model.net
-        if (self.FUSED_SAMPLER and 4 * bs * self.action_pred_steps <= 12 and self.action_pred_steps == 3
-                and net.x_embedder.linear.weight.shape[0] in (64 * net.num_heads, 96 * net.num_heads)
-                and not torch.is_grad_enabled()):
+        if self._fused_sampler_fits(bs):
             # one sequence (rollouts): the whole guided DDIM loop as one persistent kernel (csrc/dit_sampler.cu)
             from .. import _lib as L
             return L.dit_ddim_sample(net, self.action_model.ddim_diffusion, feat.to(torch.bfloat16), noise[:bs].float(),

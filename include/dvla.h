@@ -284,7 +284,18 @@ int dvla_grad_clip_scale(void* g_bf16, int64_t n, const float* sumsq, float max_
  * rows = 2 * batch * 2T <= 24).  Every pointer is device memory, weights are bf16 nn.Linear layouts [out, in].
  * head_dim = hidden / heads must be 64 (DiT-B, DiT-L) or 96 (DiT-S); DVLA_ERR_UNSUPPORTED otherwise.
  * Schedule tables are HOST arrays of n_steps entries (respaced DDIM: timestep_map[i] is the original timestep of step i).
+ * n_steps <= 12 (the prologue embeds every step's timestep as one row of a 12-row GEMM); DVLA_ERR_UNSUPPORTED otherwise.
+ *
+ * integrator (appended after version 100 shipped; 0 means DDIM, so zero-initialised structs keep their meaning):
+ *   DVLA_DIT_DDIM     the eta = 0 DDIM update over timestep_map / the alpha tables, steps n_steps-1 .. 0; the start noise
+ *                     is rounded to bf16 first (the module path casts it to the model dtype).
+ *   DVLA_DIT_FM_EULER flow matching (`--use_fm`, FMDiffusion.ddim_sample_loop): steps 0 .. n_steps-1, the DiT's timestep
+ *                     input of step i is t_values[i] (fp32, i / n_steps), the start state is the fp32 `noise` as given and
+ *                     x += bf16((1 / n_steps) * u) with u the bf16 guided output.  timestep_map and the alpha tables are
+ *                     not read (may be NULL); the module path forces cfg_scale to 1.0, callers that mirror it pass 1.0.
+ *   Any other value returns DVLA_ERR_UNSUPPORTED, DVLA_DIT_FM_EULER with t_values NULL DVLA_ERR_INVALID, before any launch.
  * ------------------------------------------------------------------------------------------------------------- */
+enum { DVLA_DIT_DDIM = 0, DVLA_DIT_FM_EULER = 1 };
 typedef struct {
   const void *qkv_w, *qkv_b, *proj_w, *proj_b, *fc1_w, *fc1_b, *fc2_w, *fc2_b;   /* blocks.N.{attn.qkv, attn.proj, mlp.fc1, mlp.fc2} */
 } dvla_dit_block_weights;
@@ -297,13 +308,15 @@ typedef struct {
   const void *pos;                       /* positional_embedding [2T, hidden] */
   const void *final_w, *final_b;         /* final_layer.linear [channels, hidden], [channels] */
   const void* z;                         /* bf16 [batch, T, token]: condition features (the backbone's action-token rows) */
-  const float* noise;                    /* fp32 [batch, T, channels]: DDIM start noise */
+  const float* noise;                    /* fp32 [batch, T, channels]: start state (DDIM noise, or the FM start state) */
   float* out;                            /* fp32 [batch, T, channels] */
   const int32_t* timestep_map;           /* HOST [n_steps] */
   const float *sqrt_recip_alphas_cumprod, *sqrt_recipm1_alphas_cumprod, *alphas_cumprod_prev;   /* HOST [n_steps] */
   int64_t n_steps;
   float cfg_scale;
   void* workspace; int64_t workspace_bytes;   /* >= dvla_dit_sampler_workspace_bytes(...) */
+  int64_t integrator;                    /* DVLA_DIT_DDIM (0) or DVLA_DIT_FM_EULER (1), see above */
+  const float* t_values;                 /* HOST [n_steps]: DiT timestep input of each step in execution order (FM only) */
 } dvla_dit_sampler_args;
 int64_t dvla_dit_sampler_workspace_bytes(int64_t batch, int64_t T, int64_t hidden, int64_t mlp, int64_t n_steps);
 int dvla_dit_ddim_sample(const dvla_dit_sampler_args* args, void* stream);

@@ -1,4 +1,6 @@
 """Timing of the action sampler alone: fused megakernel (csrc/dit_sampler.cu) vs the module path, batch 1 and 2.
+At batch 2 the FUSED_SAMPLER run is also the module path (two sequences are 24 rows, the kernel takes 12), called eagerly
+instead of replayed as a graph: that row measures launch overhead, not the kernel.
    python tools/prof_sampler.py"""
 import os
 import sys
@@ -41,5 +43,6 @@ for bs in (1, 2):
                 run()
             e1.record()
             torch.cuda.synchronize()
-        print(f"sampler bs={bs} {'fused megakernel' if fused else 'module path (graph replay)'}: {e0.elapsed_time(e1) / 10:.3f} ms",
+        label = "module path (graph replay)" if not fused else "fused megakernel" if bs == 1 else "module path (eager)"
+        print(f"sampler bs={bs} {label}: {e0.elapsed_time(e1) / 10:.3f} ms",
               flush=True)
