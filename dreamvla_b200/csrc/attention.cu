@@ -948,7 +948,7 @@ attn_mask_obs_drop_kernel(const uint32_t* __restrict__ base, uint32_t* __restric
 
 // ===================================================== host =======================================================
 static bool strides_ok(const void* ptr, long long sb, long long ss, long long sh) {
-  return ptr && (reinterpret_cast<uintptr_t>(ptr) % 16 == 0) && sb % 8 == 0 && ss % 8 == 0 && sh % 8 == 0;
+  return ptr && aligned16(ptr) && sb % 8 == 0 && ss % 8 == 0 && sh % 8 == 0;
 }
 
 bool attn_small_applicable(int64_t Lq, int64_t Lk, const void* mask, float dropout_p);   // attention_small.cu

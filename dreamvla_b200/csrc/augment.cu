@@ -68,12 +68,6 @@ __global__ void __launch_bounds__(256) resize_nearest_kernel(const float* __rest
   }
 }
 
-static unsigned grid_for(long long total) {
-  long long blocks = (total + 255) / 256;
-  const long long cap = 32LL * num_sms();
-  return static_cast<unsigned>(blocks < cap ? (blocks > 0 ? blocks : 1) : cap);
-}
-
 // ---- image_fn ----------------------------------------------------------------------------------------------------------------
 constexpr int kCrop = 224;                 // CLIP ViT input side
 constexpr int kPrecisionBits = 22;         // Pillow Resample.c PRECISION_BITS = 32 - 8 - 2
@@ -218,7 +212,7 @@ extern "C" int dvla_shift_crop(const void* x, void* out, const int32_t* shifts, 
   if (!x || !out || !shifts) { set_error("shift_crop: null pointer"); return DVLA_ERR_INVALID; }
   if (n < 0 || c <= 0 || h <= 0 || w <= 0 || pad < 0 || h > 32768 || w > 32768 || c > 65535) { set_error("shift_crop: bad dims"); return DVLA_ERR_INVALID; }
   if ((in_dtype | out_dtype) & ~1) { set_error("shift_crop: dtype codes are 0 (fp32) / 1 (bf16)"); return DVLA_ERR_INVALID; }
-  const unsigned g = grid_for(n * c * h * 32);          // one warp per row
+  const unsigned g = grid_for(n * c * h * 32, 256, 32);   // one warp per row
 #define SC(TI, TO) shift_crop_kernel<TI, TO><<<g, 256, 0, s>>>((const TI*)x, (TO*)out, shifts, n, (int)c, (int)h, (int)w, pad)
   switch (in_dtype * 2 + out_dtype) {
     case 0: SC(float, float); break;
@@ -242,7 +236,7 @@ extern "C" int dvla_resize_nearest(const float* x, void* out, int64_t n, int64_t
   if (out_dtype & ~1) { set_error("resize_nearest: dtype codes are 0 (fp32) / 1 (bf16)"); return DVLA_ERR_INVALID; }
   if (n == 0) return DVLA_OK;
   const float sh = static_cast<float>(hin) / static_cast<float>(hout), sw = static_cast<float>(win) / static_cast<float>(wout);
-  const unsigned g = grid_for(n * hout * wout);
+  const unsigned g = grid_for(n * hout * wout, 256, 32);
   if (out_dtype == 0) resize_nearest_kernel<float><<<g, 256, 0, s>>>(x, (float*)out, n, (int)hin, (int)win, (int)hout, (int)wout, sh, sw);
   else                resize_nearest_kernel<bf16><<<g, 256, 0, s>>>(x, (bf16*)out, n, (int)hin, (int)win, (int)hout, (int)wout, sh, sw);
   DVLA_CHECK_LAUNCH("resize_nearest");
@@ -303,7 +297,7 @@ extern "C" int dvla_image_fn(const dvla_image_fn_args* a, void* stream) {
     return DVLA_ERR_INVALID;
   }
   if (a->out_dtype & ~1) { set_error("image_fn: dtype codes are 0 (fp32) / 1 (bf16)"); return DVLA_ERR_INVALID; }
-  if ((reinterpret_cast<uintptr_t>(a->out) & 15) != 0) { set_error("image_fn: out must be 16-byte aligned"); return DVLA_ERR_INVALID; }
+  if (!aligned16(a->out)) { set_error("image_fn: out must be 16-byte aligned"); return DVLA_ERR_INVALID; }
   int64_t rh, rw, top, left;
   image_fn_geometry(a->h, a->w, &rh, &rw, &top, &left);
   const int kx = dvla_bicubic_taps(a->w, rw), ky = dvla_bicubic_taps(a->h, rh);

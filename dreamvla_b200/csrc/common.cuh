@@ -193,6 +193,25 @@ __device__ __forceinline__ float2 unpack_bf16x2(uint32_t u) {
   __nv_bfloat162 v = *reinterpret_cast<__nv_bfloat162*>(&u);
   return __bfloat1622float2(v);
 }
+// One 16-byte vector of 8 bf16 <-> 8 fp32.  The caller issues the load or store (plain, __ldg, ld.cg, ...).
+__device__ __forceinline__ void unpack_bf16x8(const uint4& u, float (&f)[8]) {
+  float2 t;
+  t = unpack_bf16x2(u.x); f[0] = t.x; f[1] = t.y;
+  t = unpack_bf16x2(u.y); f[2] = t.x; f[3] = t.y;
+  t = unpack_bf16x2(u.z); f[4] = t.x; f[5] = t.y;
+  t = unpack_bf16x2(u.w); f[6] = t.x; f[7] = t.y;
+}
+__device__ __forceinline__ uint4 pack_bf16x8(const float (&f)[8]) {
+  return make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]), pack_bf16x2(f[6], f[7]));
+}
+// The same with a plain 16-byte load / store at p (16-byte aligned).  The load goes to a local first: a reference bound to
+// the memory itself would let the compiler split it into four 4-byte loads.
+__device__ __forceinline__ void load_bf16x8(const bf16* p, float (&f)[8]) {
+  const uint4 u = *reinterpret_cast<const uint4*>(p);
+  unpack_bf16x8(u, f);
+}
+__device__ __forceinline__ void store_bf16x8(bf16* p, const float (&f)[8]) { *reinterpret_cast<uint4*>(p) = pack_bf16x8(f); }
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -54,18 +54,6 @@ struct DitSamplerParams {
   float fm_delta;            // Euler step 1 / n_steps
 };
 
-__device__ __forceinline__ float warp_sum_f(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-__device__ __forceinline__ void unpack8(const uint4& u, float (&f)[8]) {
-  float2 t;
-  t = unpack_bf16x2(u.x); f[0] = t.x; f[1] = t.y;
-  t = unpack_bf16x2(u.y); f[2] = t.x; f[3] = t.y;
-  t = unpack_bf16x2(u.z); f[4] = t.x; f[5] = t.y;
-  t = unpack_bf16x2(u.w); f[6] = t.x; f[7] = t.y;
-}
 __device__ __forceinline__ float gelu_tanh_f(float x) {
   const float u = 0.7978845608028654f * (x + 0.044715f * x * x * x);
   return 0.5f * x * (1.0f + tanhf(u));
@@ -107,11 +95,11 @@ __device__ __noinline__ void skinny_gemm(const bf16* __restrict__ Xs, int M, int
           const int c = c0 + 32 * u;
           if (c >= ce) continue;
           float wa[8];
-          unpack8(a[u], wa);
+          unpack_bf16x8(a[u], wa);
 #pragma unroll
           for (int m = 0; m < MROWS; ++m) {
             float x[8];
-            unpack8(*reinterpret_cast<const uint4*>(Xs + (m < M ? m : 0) * K + c * 8), x);
+            unpack_bf16x8(*reinterpret_cast<const uint4*>(Xs + (m < M ? m : 0) * K + c * 8), x);
             float s0 = 0.f;
 #pragma unroll
             for (int j = 0; j < 8; ++j) s0 = fmaf(x[j], wa[j], s0);
@@ -152,12 +140,12 @@ __device__ __noinline__ void skinny_gemm(const bf16* __restrict__ Xs, int M, int
         const int c = c0 + 32 * u;
         if (c >= chunks) continue;
         float wa[8], wb[8];
-        unpack8(a[u], wa);
-        unpack8(b[u], wb);
+        unpack_bf16x8(a[u], wa);
+        unpack_bf16x8(b[u], wb);
 #pragma unroll
         for (int m = 0; m < MROWS; ++m) {
           float x[8];
-          unpack8(*reinterpret_cast<const uint4*>(Xs + (m < M ? m : 0) * K + c * 8), x);
+          unpack_bf16x8(*reinterpret_cast<const uint4*>(Xs + (m < M ? m : 0) * K + c * 8), x);
           float s0 = 0.f, s1 = 0.f;
 #pragma unroll
           for (int j = 0; j < 8; ++j) { s0 = fmaf(x[j], wa[j], s0); s1 = fmaf(x[j], wb[j], s1); }
@@ -210,7 +198,7 @@ __device__ __forceinline__ void stage_layernorm_row(bf16* __restrict__ dst, cons
   float s = 0.f;
 #pragma unroll
   for (int u = 0; u < 8; ++u) s += (v[u].x + v[u].y) + (v[u].z + v[u].w);
-  const float mean = warp_sum_f(s) / H;
+  const float mean = warp_sum(s) / H;
   float q = 0.f;
 #pragma unroll
   for (int u = 0; u < 8; ++u) {
@@ -219,7 +207,7 @@ __device__ __forceinline__ void stage_layernorm_row(bf16* __restrict__ dst, cons
       q += (a * a + b * b) + (c * c + d * d);
     }
   }
-  const float rstd = rsqrtf(warp_sum_f(q) / H + 1e-6f);
+  const float rstd = rsqrtf(warp_sum(q) / H + 1e-6f);
   uint2* d2 = reinterpret_cast<uint2*>(dst);
 #pragma unroll
   for (int u = 0; u < 8; ++u) {
@@ -409,7 +397,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dit_ddim_sample_kernel(const __
         const int r = o / C, cc = o - r * C;
         float s = 0.f;
         for (int c = lane; c < H; c += 32) s = fmaf(__bfloat162float(Xs[r * H + c]), __bfloat162float(p.fin_w[cc * H + c]), s);
-        s = warp_sum_f(s);
+        s = warp_sum(s);
         if (lane == 0) eps_s[o] = __bfloat162float(__float2bfloat16(s + __bfloat162float(p.fin_b[cc])));
       }
       __syncthreads();

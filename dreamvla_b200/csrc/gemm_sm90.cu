@@ -732,15 +732,13 @@ static bool splitk_enabled() {
   return on;
 }
 
-static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-
 // workspace = [16384 arrival counters (64 KB), zero between launches] [fp32 partial tiles: 128 x 128 x 4 bytes per CTA and split]
 constexpr int64_t TAIL_CNT_BYTES = 65536;
 constexpr int64_t TAIL_WS_SLICES = 132;              // 128 x 128 fp32 slices (8.25 MB): a split tail wave needs <= 132 (one
                                                      // per SM)
 
 static bool tail_fits(const dvla_gemm_args* a, long long tail_tiles, int splits) {
-  if (!a->workspace || (reinterpret_cast<uintptr_t>(a->workspace) & 15)) return false;
+  if (!a->workspace || !aligned16(a->workspace)) return false;
   return tail_tiles * NUM_EPI_WARPS * 4 <= TAIL_CNT_BYTES &&
          TAIL_CNT_BYTES + tail_tiles * splits * (long long)BM * BN * 4 <= a->workspace_bytes;
 }

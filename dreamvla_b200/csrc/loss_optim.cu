@@ -17,14 +17,6 @@ __device__ __forceinline__ float block_sum_256(float v) {
   return t;  // valid in warp 0
 }
 
-static inline unsigned grid_for(long long work_items, int per_block) {
-  long long b = (work_items + per_block - 1) / per_block;
-  const long long cap = 8LL * num_sms();
-  if (b > cap) b = cap;
-  if (b < 1) b = 1;
-  return (unsigned)b;
-}
-
 // ---------------------------------------------------------------------------------------------------------------
 // MSE with optional per-row {0,1} mask:  mean((pred*m - label*m)^2) over rows*C   (train_utils.py:325-337, 499-502)
 // ---------------------------------------------------------------------------------------------------------------
@@ -160,13 +152,19 @@ __global__ void __launch_bounds__(256) sumsq_kernel(const bf16* __restrict__ g, 
   }
 }
 
-// In-place clip of the (rank-summed) accumulated gradient: g *= grad_scale * min(1, max_norm / (||g||*grad_scale + 1e-6)).
+// The factor the clip multiplies a gradient by: grad_scale * min(1, max_norm / (||g|| * grad_scale + 1e-6)), the
+// torch.nn.utils.clip_grad_norm_ semantics on a gradient that still carries the factor grad_scale.
+__device__ __forceinline__ float clip_factor(float sumsq, float max_norm, float grad_scale) {
+  const float norm = sqrtf(sumsq) * grad_scale;
+  return grad_scale * fminf(1.0f, max_norm / (norm + 1e-6f));
+}
+
+// In-place clip of the (rank-summed) accumulated gradient: g *= clip_factor.
 // Reference utils/train_utils.py:599-600 clips the ACCUMULATED gradient after every micro-step; with gradient accumulation
 // that clip must land in the buffer itself (the fused clip inside adamw_kernel only covers accumulation == 1).
 __global__ void __launch_bounds__(256) grad_clip_scale_kernel(bf16* __restrict__ g, long long n, const float* __restrict__ sumsq,
                                                               float max_norm, float grad_scale) {
-  const float norm = sqrtf(sumsq[0]) * grad_scale;
-  const float c = grad_scale * fminf(1.0f, max_norm / (norm + 1e-6f));
+  const float c = clip_factor(sumsq[0], max_norm, grad_scale);
   if (c == 1.0f) return;
   const long long nv = n >> 3;
   uint4* gv = reinterpret_cast<uint4*>(g);
@@ -189,112 +187,68 @@ struct AdamWParams {
   const float* sumsq; const float* lr; const float* step;
   float beta1, beta2, eps, wd, max_norm, grad_scale; int zero_grad;
 };
-__global__ void __launch_bounds__(256) adamw_kernel(AdamWParams a) {
-  float clip = a.grad_scale;
-  if (a.sumsq) {
-    const float norm = sqrtf(a.sumsq[0]) * a.grad_scale;
-    clip *= fminf(1.0f, a.max_norm / (norm + 1e-6f));  // torch.nn.utils.clip_grad_norm_ semantics
-  }
-  const float lr = a.lr[0];
-  const float t = a.step[0];
-  const float bc1 = 1.0f - powf(a.beta1, t);
-  const float bc2s = sqrtf(1.0f - powf(a.beta2, t));
-  const float step_size = lr / bc1;
-  const float decay = 1.0f - lr * a.wd;
-  const long long nv = a.n >> 3;
-  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < nv;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    uint4 pu = reinterpret_cast<uint4*>(a.p)[i];
-    const uint4 gu = reinterpret_cast<const uint4*>(a.g)[i];
-    float4 m0 = reinterpret_cast<float4*>(a.m)[2 * i], m1 = reinterpret_cast<float4*>(a.m)[2 * i + 1];
-    float4 v0 = reinterpret_cast<float4*>(a.v)[2 * i], v1 = reinterpret_cast<float4*>(a.v)[2 * i + 1];
-    float pf[8], gf[8], mf[8] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w},
-                        vf[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
-    float2 f;
-    f = unpack_bf16x2(pu.x); pf[0] = f.x; pf[1] = f.y; f = unpack_bf16x2(pu.y); pf[2] = f.x; pf[3] = f.y;
-    f = unpack_bf16x2(pu.z); pf[4] = f.x; pf[5] = f.y; f = unpack_bf16x2(pu.w); pf[6] = f.x; pf[7] = f.y;
-    f = unpack_bf16x2(gu.x); gf[0] = f.x; gf[1] = f.y; f = unpack_bf16x2(gu.y); gf[2] = f.x; gf[3] = f.y;
-    f = unpack_bf16x2(gu.z); gf[4] = f.x; gf[5] = f.y; f = unpack_bf16x2(gu.w); gf[6] = f.x; gf[7] = f.y;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float gj = gf[j] * clip;
-      mf[j] = a.beta1 * mf[j] + (1.0f - a.beta1) * gj;
-      vf[j] = a.beta2 * vf[j] + (1.0f - a.beta2) * gj * gj;
-      const float denom = sqrtf(vf[j]) / bc2s + a.eps;
-      pf[j] = pf[j] * decay - step_size * mf[j] / denom;
-    }
-    pu = make_uint4(pack_bf16x2(pf[0], pf[1]), pack_bf16x2(pf[2], pf[3]), pack_bf16x2(pf[4], pf[5]), pack_bf16x2(pf[6], pf[7]));
-    reinterpret_cast<uint4*>(a.p)[i] = pu;
-    reinterpret_cast<float4*>(a.m)[2 * i] = make_float4(mf[0], mf[1], mf[2], mf[3]);
-    reinterpret_cast<float4*>(a.m)[2 * i + 1] = make_float4(mf[4], mf[5], mf[6], mf[7]);
-    reinterpret_cast<float4*>(a.v)[2 * i] = make_float4(vf[0], vf[1], vf[2], vf[3]);
-    reinterpret_cast<float4*>(a.v)[2 * i + 1] = make_float4(vf[4], vf[5], vf[6], vf[7]);
-    if (a.zero_grad) reinterpret_cast<uint4*>(a.g)[i] = make_uint4(0, 0, 0, 0);
-  }
-  if (blockIdx.x == 0) {
-    for (long long i = (nv << 3) + threadIdx.x; i < a.n; i += blockDim.x) {
-      const float gj = __bfloat162float(a.g[i]) * clip;
-      const float mj = a.beta1 * a.m[i] + (1.0f - a.beta1) * gj;
-      const float vj = a.beta2 * a.v[i] + (1.0f - a.beta2) * gj * gj;
-      a.m[i] = mj; a.v[i] = vj;
-      const float denom = sqrtf(vj) / bc2s + a.eps;
-      a.p[i] = __float2bfloat16(__bfloat162float(a.p[i]) * decay - step_size * mj / denom);
-      if (a.zero_grad) a.g[i] = __float2bfloat16(0.f);
-    }
-  }
-}
-
-// The same clip + AdamW on fp32 master weights: the update lands in p32 (no bf16 rounding of the parameter between
-// steps), then the bf16 working copy the kernels read is written as round-to-nearest(p32).  Same formula and operation
-// order as adamw_kernel, except that the decay product p * (1 - lr*wd) is rounded on its own (__fmul_rn, no FMA with the
-// update), as torch.optim.AdamW's `param.mul_(1 - lr * wd)` does: at lr*wd ~ 1e-7 the decay is about one fp32 ulp of the
-// weight, and folding its rounding into the update's drifts the fp32 trajectory by ~6e-4 of the accumulated update over
-// 100 steps (2.5e-6 with the separate rounding).  The old bf16 copy is never read.  30 B per parameter (adamw_kernel: 24).
+// adamw_master_kernel: the same clip + AdamW on fp32 master weights.  The update lands in p32 (no bf16 rounding of the
+// parameter between steps), then the bf16 working copy the kernels read is written as round-to-nearest(p32).  Same formula
+// and operation order as adamw_kernel, except that the decay product p * (1 - lr*wd) is rounded on its own (__fmul_rn, no
+// FMA with the update), as torch.optim.AdamW's `param.mul_(1 - lr * wd)` does: at lr*wd ~ 1e-7 the decay is about one fp32
+// ulp of the weight, and folding its rounding into the update's drifts the fp32 trajectory by ~6e-4 of the accumulated
+// update over 100 steps (2.5e-6 with the separate rounding).  The old bf16 copy is never read.  30 B per parameter
+// (adamw_kernel: 24).
 struct AdamWMasterParams {
   float* p32; bf16* p; bf16* g; float* m; float* v; long long n;
   const float* sumsq; const float* lr; const float* step;
   float beta1, beta2, eps, wd, max_norm, grad_scale; int zero_grad;
 };
-__global__ void __launch_bounds__(256) adamw_master_kernel(AdamWMasterParams a) {
+
+__device__ __forceinline__ void load_f32x8(const float* p, long long i, float (&f)[8]) {
+  const float4 a = reinterpret_cast<const float4*>(p)[2 * i], b = reinterpret_cast<const float4*>(p)[2 * i + 1];
+  f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
+}
+__device__ __forceinline__ void store_f32x8(float* p, long long i, const float (&f)[8]) {
+  reinterpret_cast<float4*>(p)[2 * i] = make_float4(f[0], f[1], f[2], f[3]);
+  reinterpret_cast<float4*>(p)[2 * i + 1] = make_float4(f[4], f[5], f[6], f[7]);
+}
+
+// kMaster = false: P = AdamWParams, the parameter is the bf16 p.  kMaster = true: P = AdamWMasterParams, the parameter is
+// the fp32 p32 and p its bf16 copy.
+template <bool kMaster, class P>
+__device__ __forceinline__ void adamw_body(const P& a) {
   float clip = a.grad_scale;
-  if (a.sumsq) {
-    const float norm = sqrtf(a.sumsq[0]) * a.grad_scale;
-    clip *= fminf(1.0f, a.max_norm / (norm + 1e-6f));  // torch.nn.utils.clip_grad_norm_ semantics
-  }
+  if (a.sumsq) clip = clip_factor(a.sumsq[0], a.max_norm, a.grad_scale);
   const float lr = a.lr[0];
   const float t = a.step[0];
   const float bc1 = 1.0f - powf(a.beta1, t);
   const float bc2s = sqrtf(1.0f - powf(a.beta2, t));
   const float step_size = lr / bc1;
   const float decay = 1.0f - lr * a.wd;
+  auto decayed = [&](float p) {
+    if constexpr (kMaster) return __fmul_rn(p, decay);
+    else return p * decay;
+  };
   const long long nv = a.n >> 3;
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < nv;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    float pf[8], gf[8], mf[8], vf[8];
+    uint4 pu;
+    if constexpr (!kMaster) pu = reinterpret_cast<const uint4*>(a.p)[i];
     const uint4 gu = reinterpret_cast<const uint4*>(a.g)[i];
-    float4 p0 = reinterpret_cast<float4*>(a.p32)[2 * i], p1 = reinterpret_cast<float4*>(a.p32)[2 * i + 1];
-    float4 m0 = reinterpret_cast<float4*>(a.m)[2 * i], m1 = reinterpret_cast<float4*>(a.m)[2 * i + 1];
-    float4 v0 = reinterpret_cast<float4*>(a.v)[2 * i], v1 = reinterpret_cast<float4*>(a.v)[2 * i + 1];
-    float pf[8] = {p0.x, p0.y, p0.z, p0.w, p1.x, p1.y, p1.z, p1.w}, gf[8],
-          mf[8] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w}, vf[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
-    float2 f;
-    f = unpack_bf16x2(gu.x); gf[0] = f.x; gf[1] = f.y; f = unpack_bf16x2(gu.y); gf[2] = f.x; gf[3] = f.y;
-    f = unpack_bf16x2(gu.z); gf[4] = f.x; gf[5] = f.y; f = unpack_bf16x2(gu.w); gf[6] = f.x; gf[7] = f.y;
+    if constexpr (kMaster) load_f32x8(a.p32, i, pf);
+    load_f32x8(a.m, i, mf);
+    load_f32x8(a.v, i, vf);
+    if constexpr (!kMaster) unpack_bf16x8(pu, pf);
+    unpack_bf16x8(gu, gf);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const float gj = gf[j] * clip;
       mf[j] = a.beta1 * mf[j] + (1.0f - a.beta1) * gj;
       vf[j] = a.beta2 * vf[j] + (1.0f - a.beta2) * gj * gj;
       const float denom = sqrtf(vf[j]) / bc2s + a.eps;
-      pf[j] = __fmul_rn(pf[j], decay) - step_size * mf[j] / denom;
+      pf[j] = decayed(pf[j]) - step_size * mf[j] / denom;
     }
-    reinterpret_cast<float4*>(a.p32)[2 * i] = make_float4(pf[0], pf[1], pf[2], pf[3]);
-    reinterpret_cast<float4*>(a.p32)[2 * i + 1] = make_float4(pf[4], pf[5], pf[6], pf[7]);
-    reinterpret_cast<uint4*>(a.p)[i] =
-        make_uint4(pack_bf16x2(pf[0], pf[1]), pack_bf16x2(pf[2], pf[3]), pack_bf16x2(pf[4], pf[5]), pack_bf16x2(pf[6], pf[7]));
-    reinterpret_cast<float4*>(a.m)[2 * i] = make_float4(mf[0], mf[1], mf[2], mf[3]);
-    reinterpret_cast<float4*>(a.m)[2 * i + 1] = make_float4(mf[4], mf[5], mf[6], mf[7]);
-    reinterpret_cast<float4*>(a.v)[2 * i] = make_float4(vf[0], vf[1], vf[2], vf[3]);
-    reinterpret_cast<float4*>(a.v)[2 * i + 1] = make_float4(vf[4], vf[5], vf[6], vf[7]);
+    if constexpr (kMaster) store_f32x8(a.p32, i, pf);
+    reinterpret_cast<uint4*>(a.p)[i] = pack_bf16x8(pf);
+    store_f32x8(a.m, i, mf);
+    store_f32x8(a.v, i, vf);
     if (a.zero_grad) reinterpret_cast<uint4*>(a.g)[i] = make_uint4(0, 0, 0, 0);
   }
   if (blockIdx.x == 0) {
@@ -304,13 +258,18 @@ __global__ void __launch_bounds__(256) adamw_master_kernel(AdamWMasterParams a) 
       const float vj = a.beta2 * a.v[i] + (1.0f - a.beta2) * gj * gj;
       a.m[i] = mj; a.v[i] = vj;
       const float denom = sqrtf(vj) / bc2s + a.eps;
-      const float pj = __fmul_rn(a.p32[i], decay) - step_size * mj / denom;
-      a.p32[i] = pj;
-      a.p[i] = __float2bfloat16_rn(pj);
+      float pj;
+      if constexpr (kMaster) pj = a.p32[i];
+      else pj = __bfloat162float(a.p[i]);
+      pj = decayed(pj) - step_size * mj / denom;
+      if constexpr (kMaster) a.p32[i] = pj;
+      a.p[i] = __float2bfloat16(pj);
       if (a.zero_grad) a.g[i] = __float2bfloat16(0.f);
     }
   }
 }
+__global__ void __launch_bounds__(256) adamw_kernel(AdamWParams a) { adamw_body<false>(a); }
+__global__ void __launch_bounds__(256) adamw_master_kernel(AdamWMasterParams a) { adamw_body<true>(a); }
 
 }  // namespace dvla
 
@@ -321,7 +280,7 @@ extern "C" int dvla_mse_loss(const void* pred, const void* label, const float* r
   const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (!pred || !label || !loss_out) { set_error("mse_loss: null pointer"); return DVLA_ERR_INVALID; }
   if (rows <= 0 || C <= 0) return DVLA_OK;
-  mse_loss_kernel<<<grid_for(rows * C, 256 * 8), 256, 0, s>>>((const bf16*)pred, (const bf16*)label, row_mask, rows,
+  mse_loss_kernel<<<grid_for(rows * C, 256 * 8, 8), 256, 0, s>>>((const bf16*)pred, (const bf16*)label, row_mask, rows,
                                                              (int)C, weight, loss_out, (bf16*)dpred);
   DVLA_CHECK_LAUNCH("mse_loss");
   return DVLA_OK;
@@ -332,7 +291,7 @@ extern "C" int dvla_cosine_loss(const void* pred, const void* label, int64_t row
   const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (!pred || !label || !loss_out) { set_error("cosine_loss: null pointer"); return DVLA_ERR_INVALID; }
   if (rows <= 0 || C <= 0) return DVLA_OK;
-  cosine_loss_kernel<<<grid_for(rows, 8), 256, 0, s>>>((const bf16*)pred, (const bf16*)label, rows, (int)C, weight,
+  cosine_loss_kernel<<<grid_for(rows, 8, 8), 256, 0, s>>>((const bf16*)pred, (const bf16*)label, rows, (int)C, weight,
                                                       loss_out, (bf16*)dpred);
   DVLA_CHECK_LAUNCH("cosine_loss");
   return DVLA_OK;
@@ -342,7 +301,7 @@ extern "C" int dvla_silog_stats(const void* pred, const void* label, int64_t n, 
   const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (!pred || !label || !stats) { set_error("silog_stats: null pointer"); return DVLA_ERR_INVALID; }
   if (n <= 0) return DVLA_OK;
-  silog_stats_kernel<<<grid_for(n, 256 * 8), 256, 0, s>>>((const bf16*)pred, (const bf16*)label, n, stats);
+  silog_stats_kernel<<<grid_for(n, 256 * 8, 8), 256, 0, s>>>((const bf16*)pred, (const bf16*)label, n, stats);
   DVLA_CHECK_LAUNCH("silog_stats");
   return DVLA_OK;
 }
@@ -352,7 +311,7 @@ extern "C" int dvla_silog_finish(const void* pred, const void* label, int64_t n,
   const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (!pred || !label || !stats || !loss_out) { set_error("silog_finish: null pointer"); return DVLA_ERR_INVALID; }
   if (n <= 0) return DVLA_OK;
-  silog_finish_kernel<<<grid_for(n, 256 * 8), 256, 0, s>>>((const bf16*)pred, (const bf16*)label, n, stats, lambd, weight,
+  silog_finish_kernel<<<grid_for(n, 256 * 8, 8), 256, 0, s>>>((const bf16*)pred, (const bf16*)label, n, stats, lambd, weight,
                                                           loss_out, (bf16*)dpred);
   DVLA_CHECK_LAUNCH("silog_finish");
   return DVLA_OK;
@@ -362,9 +321,9 @@ extern "C" int64_t dvla_silog_workspace_bytes(void) { return 2 * (int64_t)sizeof
 extern "C" int dvla_sumsq(const void* g, int64_t n, float* out, void* stream) {
   const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (!g || !out) { set_error("sumsq: null pointer"); return DVLA_ERR_INVALID; }
-  if (reinterpret_cast<uintptr_t>(g) & 15) { set_error("sumsq: buffer must be 16-byte aligned"); return DVLA_ERR_INVALID; }
+  if (!aligned16(g)) { set_error("sumsq: buffer must be 16-byte aligned"); return DVLA_ERR_INVALID; }
   if (n <= 0) return DVLA_OK;
-  unsigned blocks = grid_for(n, 256 * 8 * 4);
+  unsigned blocks = grid_for(n, 256 * 8 * 4, 8);
   if (blocks > SUMSQ_MAX_BLOCKS) blocks = SUMSQ_MAX_BLOCKS;
   sumsq_kernel<<<blocks, 256, 0, s>>>((const bf16*)g, n, out);
   DVLA_CHECK_LAUNCH("sumsq");
@@ -374,9 +333,9 @@ extern "C" int dvla_sumsq(const void* g, int64_t n, float* out, void* stream) {
 extern "C" int dvla_grad_clip_scale(void* g, int64_t n, const float* sumsq, float max_norm, float grad_scale, void* stream) {
   const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (!g || !sumsq) { set_error("grad_clip_scale: null pointer"); return DVLA_ERR_INVALID; }
-  if (reinterpret_cast<uintptr_t>(g) & 15) { set_error("grad_clip_scale: buffer must be 16-byte aligned"); return DVLA_ERR_INVALID; }
+  if (!aligned16(g)) { set_error("grad_clip_scale: buffer must be 16-byte aligned"); return DVLA_ERR_INVALID; }
   if (n <= 0) return DVLA_OK;
-  grad_clip_scale_kernel<<<grid_for(n, 256 * 8 * 4), 256, 0, s>>>((bf16*)g, n, sumsq, max_norm, grad_scale);
+  grad_clip_scale_kernel<<<grid_for(n, 256 * 8 * 4, 8), 256, 0, s>>>((bf16*)g, n, sumsq, max_norm, grad_scale);
   DVLA_CHECK_LAUNCH("grad_clip_scale");
   return DVLA_OK;
 }
@@ -384,12 +343,11 @@ extern "C" int dvla_grad_clip_scale(void* g, int64_t n, const float* sumsq, floa
 extern "C" int dvla_adamw(const dvla_adamw_args* a, void* stream) {
   const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (!a || !a->p || !a->g || !a->m || !a->v || !a->lr || !a->step) { set_error("adamw: null pointer"); return DVLA_ERR_INVALID; }
-  if ((reinterpret_cast<uintptr_t>(a->p) | reinterpret_cast<uintptr_t>(a->g) | reinterpret_cast<uintptr_t>(a->m) |
-       reinterpret_cast<uintptr_t>(a->v)) & 15) { set_error("adamw: buffers must be 16-byte aligned"); return DVLA_ERR_INVALID; }
+  if (!aligned16(a->p, a->g, a->m, a->v)) { set_error("adamw: buffers must be 16-byte aligned"); return DVLA_ERR_INVALID; }
   if (a->n <= 0) return DVLA_OK;
   AdamWParams k{(bf16*)a->p, (bf16*)a->g, a->m, a->v, a->n, a->sumsq, a->lr, a->step,
                 a->beta1, a->beta2, a->eps, a->weight_decay, a->max_norm, a->grad_scale, a->zero_grad};
-  adamw_kernel<<<grid_for(a->n, 256 * 8 * 2), 256, 0, s>>>(k);
+  adamw_kernel<<<grid_for(a->n, 256 * 8 * 2, 8), 256, 0, s>>>(k);
   DVLA_CHECK_LAUNCH("adamw");
   return DVLA_OK;
 }
@@ -400,15 +358,14 @@ extern "C" int dvla_adamw_master(const dvla_adamw_master_args* a, void* stream) 
     set_error("adamw_master: null pointer");
     return DVLA_ERR_INVALID;
   }
-  if ((reinterpret_cast<uintptr_t>(a->p32) | reinterpret_cast<uintptr_t>(a->p) | reinterpret_cast<uintptr_t>(a->g) |
-       reinterpret_cast<uintptr_t>(a->m) | reinterpret_cast<uintptr_t>(a->v)) & 15) {
+  if (!aligned16(a->p32, a->p, a->g, a->m, a->v)) {
     set_error("adamw_master: buffers must be 16-byte aligned");
     return DVLA_ERR_INVALID;
   }
   if (a->n <= 0) return DVLA_OK;
   AdamWMasterParams k{a->p32, (bf16*)a->p, (bf16*)a->g, a->m, a->v, a->n, a->sumsq, a->lr, a->step,
                       a->beta1, a->beta2, a->eps, a->weight_decay, a->max_norm, a->grad_scale, a->zero_grad};
-  adamw_master_kernel<<<grid_for(a->n, 256 * 8 * 2), 256, 0, s>>>(k);
+  adamw_master_kernel<<<grid_for(a->n, 256 * 8 * 2, 8), 256, 0, s>>>(k);
   DVLA_CHECK_LAUNCH("adamw_master");
   return DVLA_OK;
 }

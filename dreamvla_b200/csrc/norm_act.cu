@@ -6,19 +6,6 @@
 
 namespace dvla {
 
-__device__ __forceinline__ void load8(const bf16* p, float (&f)[8]) {
-  uint4 u = *reinterpret_cast<const uint4*>(p);
-  float2 t;
-  t = unpack_bf16x2(u.x); f[0] = t.x; f[1] = t.y;
-  t = unpack_bf16x2(u.y); f[2] = t.x; f[3] = t.y;
-  t = unpack_bf16x2(u.z); f[4] = t.x; f[5] = t.y;
-  t = unpack_bf16x2(u.w); f[6] = t.x; f[7] = t.y;
-}
-__device__ __forceinline__ void store8(bf16* p, const float (&f)[8]) {
-  *reinterpret_cast<uint4*>(p) =
-      make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]), pack_bf16x2(f[6], f[7]));
-}
-
 // ------------------------------------------------------------------------------------------------------------------
 // LayerNorm forward: warp per row; row cached in registers (D <= 1024) => one HBM read + one write per element.
 // ------------------------------------------------------------------------------------------------------------------
@@ -37,7 +24,7 @@ __global__ void __launch_bounds__(256) layernorm_fwd_kernel(const bf16* __restri
     for (int i = 0; i < NV; ++i) {
       const int vi = lane + i * 32;
       if (vi < nvec) {
-        load8(xr + vi * 8, v[i]);
+        load_bf16x8(xr + vi * 8, v[i]);
 #pragma unroll
         for (int j = 0; j < 8; ++j) s += v[i][j];
       } else {
@@ -67,8 +54,8 @@ __global__ void __launch_bounds__(256) layernorm_fwd_kernel(const bf16* __restri
       if (vi < nvec) {
         float o[8];
         float gm[8], bt[8];
-        if (gamma) load8(gamma + vi * 8, gm);
-        if (beta) load8(beta + vi * 8, bt);
+        if (gamma) load_bf16x8(gamma + vi * 8, gm);
+        if (beta) load_bf16x8(beta + vi * 8, bt);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           float t = (v[i][j] - mean) * rstd;
@@ -76,7 +63,7 @@ __global__ void __launch_bounds__(256) layernorm_fwd_kernel(const bf16* __restri
           if (beta) t += bt[j];
           o[j] = t;
         }
-        store8(yr + vi * 8, o);
+        store_bf16x8(yr + vi * 8, o);
       }
     }
   }
@@ -101,13 +88,6 @@ __global__ void __launch_bounds__(256, 2) layernorm_bwd_kernel(const bf16* __res
 #pragma unroll
     for (int j = 0; j < 8; ++j) { pg[i][j] = 0.f; pb[i][j] = 0.f; }
 
-  auto unpack8 = [](const uint4& u, float (&f)[8]) {
-    float2 t;
-    t = unpack_bf16x2(u.x); f[0] = t.x; f[1] = t.y;
-    t = unpack_bf16x2(u.y); f[2] = t.x; f[3] = t.y;
-    t = unpack_bf16x2(u.z); f[4] = t.x; f[5] = t.y;
-    t = unpack_bf16x2(u.w); f[6] = t.x; f[7] = t.y;
-  };
   // The row is kept as the RAW bf16 vectors it was loaded as (8 registers per 16 B of x and dy instead of 16 fp32) and
   // unpacked twice: with the dgamma/dbeta partials that fits 128 registers, i.e. two CTAs per SM and twice the loads in
   // flight of this latency-bound, HBM-limited kernel.
@@ -131,9 +111,9 @@ __global__ void __launch_bounds__(256, 2) layernorm_bwd_kernel(const bf16* __res
       const int vi = lane + i * 32;
       if (vi < nvec) {
         float xv[8], dv[8], gm[8];
-        unpack8(xr[i], xv);
-        unpack8(dr[i], dv);
-        if (gamma) load8(gamma + vi * 8, gm);
+        unpack_bf16x8(xr[i], xv);
+        unpack_bf16x8(dr[i], dv);
+        if (gamma) load_bf16x8(gamma + vi * 8, gm);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           const float h = (xv[j] - mu) * rs;
@@ -152,9 +132,9 @@ __global__ void __launch_bounds__(256, 2) layernorm_bwd_kernel(const bf16* __res
       const int vi = lane + i * 32;
       if (vi < nvec) {
         float xv[8], dv[8], gm[8], o[8];
-        unpack8(xr[i], xv);
-        unpack8(dr[i], dv);
-        if (gamma) load8(gamma + vi * 8, gm);
+        unpack_bf16x8(xr[i], xv);
+        unpack_bf16x8(dr[i], dv);
+        if (gamma) load_bf16x8(gamma + vi * 8, gm);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           const float h = (xv[j] - mu) * rs;
@@ -163,11 +143,11 @@ __global__ void __launch_bounds__(256, 2) layernorm_bwd_kernel(const bf16* __res
         }
         if (dres) {                                   // + gradient of the residual branch that forked at x
           float r8[8];
-          load8(dres + row * ld + vi * 8, r8);
+          load_bf16x8(dres + row * ld + vi * 8, r8);
 #pragma unroll
           for (int j = 0; j < 8; ++j) o[j] += r8[j];
         }
-        store8(dx + row * ld + vi * 8, o);
+        store_bf16x8(dx + row * ld + vi * 8, o);
       }
     }
   }
@@ -214,15 +194,8 @@ __global__ void __launch_bounds__(256, 2) layernorm_bwd_v2_kernel(const bf16* __
   float* ab = ag + D;
   for (int i = lane; i < 2 * D; i += 32) ag[i] = 0.f;
   __syncwarp();
-  auto unpack8 = [](const uint4& u, float (&f)[8]) {
-    float2 t;
-    t = unpack_bf16x2(u.x); f[0] = t.x; f[1] = t.y;
-    t = unpack_bf16x2(u.y); f[2] = t.x; f[3] = t.y;
-    t = unpack_bf16x2(u.z); f[4] = t.x; f[5] = t.y;
-    t = unpack_bf16x2(u.w); f[6] = t.x; f[7] = t.y;
-  };
   auto load_gamma = [&](int i, float (&g)[8]) {       // 2 KB, L1 resident: cheaper than 8 * NV registers per lane
-    if (gamma) load8(gamma + (lane + i * 32) * 8, g);
+    if (gamma) load_bf16x8(gamma + (lane + i * 32) * 8, g);
     else {
 #pragma unroll
       for (int j = 0; j < 8; ++j) g[j] = 1.f;
@@ -242,8 +215,8 @@ __global__ void __launch_bounds__(256, 2) layernorm_bwd_v2_kernel(const bf16* __
 #pragma unroll
     for (int i = 0; i < NV; ++i) {
       float xv[8], dv[8], gmv[8];
-      unpack8(xr[i], xv);
-      unpack8(dr[i], dv);
+      unpack_bf16x8(xr[i], xv);
+      unpack_bf16x8(dr[i], dv);
       load_gamma(i, gmv);
       const int c0 = (lane + i * 32) * 8;
       float4 g0 = *reinterpret_cast<float4*>(ag + c0), g1 = *reinterpret_cast<float4*>(ag + c0 + 4);
@@ -268,16 +241,16 @@ __global__ void __launch_bounds__(256, 2) layernorm_bwd_v2_kernel(const bf16* __
 #pragma unroll
     for (int i = 0; i < NV; ++i) {
       float xv[8], dv[8], r8[8], o[8], gmv[8];
-      unpack8(xr[i], xv);
-      unpack8(dr[i], dv);
-      unpack8(rr[i], r8);
+      unpack_bf16x8(xr[i], xv);
+      unpack_bf16x8(dr[i], dv);
+      unpack_bf16x8(rr[i], r8);
       load_gamma(i, gmv);
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         const float h = (xv[j] - mu) * rs;
         o[j] = fmaf(rs, dv[j] * gmv[j] - s1 - h * s2, r8[j]);
       }
-      store8(dx + row * ld + (lane + i * 32) * 8, o);
+      store_bf16x8(dx + row * ld + (lane + i * 32) * 8, o);
     }
   }
   __syncthreads();
@@ -322,7 +295,7 @@ __global__ void __launch_bounds__(256) colsum_kernel(const bf16* __restrict__ x,
       }
       for (; r < r1; r += 8) {
         float f[8];
-        load8(x + r * ld + col, f);
+        load_bf16x8(x + r * ld + col, f);
 #pragma unroll
         for (int j = 0; j < 8; ++j) acc[j] += f[j];
       }
@@ -369,10 +342,10 @@ __global__ void dropout_kernel(const bf16* __restrict__ x, bf16* __restrict__ y,
     const uint32_t keep = dropout_keep8(seed, static_cast<uint64_t>(i), thresh);
     if (vec) {
       float f[8];
-      load8(x + row * ldx + col, f);
+      load_bf16x8(x + row * ldx + col, f);
 #pragma unroll
       for (int j = 0; j < 8; ++j) f[j] = ((keep >> j) & 1u) ? f[j] * scale : 0.f;
-      store8(y + row * ldy + col, f);
+      store_bf16x8(y + row * ldy + col, f);
     } else {
       for (int j = 0; j < 8 && col + j < N; ++j) {
         const float f = __bfloat162float(x[row * ldx + col + j]);
@@ -393,15 +366,11 @@ __global__ void __launch_bounds__(256) act_bwd_kernel(const bf16* __restrict__ d
   const uint4* pre4 = reinterpret_cast<const uint4*>(pre);
   uint4* dx4 = reinterpret_cast<uint4*>(dx);
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < nvec; i += stride) {
-    const uint4 a = __ldg(dy4 + i), b = __ldg(pre4 + i);
     float v[8], x[8];
-    float2 f;
-    f = unpack_bf16x2(a.x); v[0] = f.x; v[1] = f.y; f = unpack_bf16x2(a.y); v[2] = f.x; v[3] = f.y;
-    f = unpack_bf16x2(a.z); v[4] = f.x; v[5] = f.y; f = unpack_bf16x2(a.w); v[6] = f.x; v[7] = f.y;
-    f = unpack_bf16x2(b.x); x[0] = f.x; x[1] = f.y; f = unpack_bf16x2(b.y); x[2] = f.x; x[3] = f.y;
-    f = unpack_bf16x2(b.z); x[4] = f.x; x[5] = f.y; f = unpack_bf16x2(b.w); x[6] = f.x; x[7] = f.y;
+    unpack_bf16x8(__ldg(dy4 + i), v);
+    unpack_bf16x8(__ldg(pre4 + i), x);
     act_bwd_mul_n<8>(v, x, act);
-    dx4[i] = make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
+    dx4[i] = pack_bf16x8(v);
   }
   for (long long i = (nvec << 3) + static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride)
     dx[i] = __float2bfloat16(__bfloat162float(dy[i]) * act_bwd(__bfloat162float(pre[i]), act));
@@ -431,16 +400,12 @@ __global__ void __launch_bounds__(256) act_bwd_colsum_kernel(const bf16* __restr
   float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   auto one = [&](const uint4& a, const uint4& b, long long r) {
     float v[8], x[8];
-    float2 f;
-    f = unpack_bf16x2(a.x); v[0] = f.x; v[1] = f.y; f = unpack_bf16x2(a.y); v[2] = f.x; v[3] = f.y;
-    f = unpack_bf16x2(a.z); v[4] = f.x; v[5] = f.y; f = unpack_bf16x2(a.w); v[6] = f.x; v[7] = f.y;
-    f = unpack_bf16x2(b.x); x[0] = f.x; x[1] = f.y; f = unpack_bf16x2(b.y); x[2] = f.x; x[3] = f.y;
-    f = unpack_bf16x2(b.z); x[4] = f.x; x[5] = f.y; f = unpack_bf16x2(b.w); x[6] = f.x; x[7] = f.y;
+    unpack_bf16x8(a, v);
+    unpack_bf16x8(b, x);
     act_bwd_mul_n<8>(v, x, act);
 #pragma unroll
     for (int j = 0; j < 8; ++j) acc[j] += v[j];
-    *reinterpret_cast<uint4*>(dx + r * N + col) =
-        make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
+    store_bf16x8(dx + r * N + col, v);
   };
   if (col < N) {
     long long r = r0 + warp;
@@ -483,6 +448,17 @@ __global__ void __launch_bounds__(256) cat_broadcast_kernel(const uint4* __restr
   }
 }
 
+// Calls f(std::integral_constant<int, NV>()) for the LayerNorm kernels' NV = ceil(D / 256) in 1..4 (D <= 1024).
+template <class F>
+static auto with_nv(int nv, F f) {
+  switch (nv) {
+    case 1: return f(std::integral_constant<int, 1>());
+    case 2: return f(std::integral_constant<int, 2>());
+    case 3: return f(std::integral_constant<int, 3>());
+    default: return f(std::integral_constant<int, 4>());
+  }
+}
+
 }  // namespace dvla
 
 using namespace dvla;
@@ -495,14 +471,11 @@ extern "C" int dvla_layernorm_fwd(const dvla_layernorm_fwd_args* a, void* stream
     return DVLA_ERR_UNSUPPORTED;
   }
   if (a->rows <= 0) return DVLA_OK;
-  const int nv = (int)((a->D + 255) / 256);
-  long long blocks = (a->rows + 7) / 8;
-  const long long cap = (long long)num_sms() * 8;
-  if (blocks > cap) blocks = cap;
-#define LN_FWD(NV) layernorm_fwd_kernel<NV><<<(unsigned)blocks, 256, 0, s>>>((const bf16*)a->x, (const bf16*)a->gamma, \
-      (const bf16*)a->beta, (bf16*)a->y, a->mean, a->rstd, a->rows, (int)a->D, a->ldx, a->ldy, a->eps)
-  switch (nv) { case 1: LN_FWD(1); break; case 2: LN_FWD(2); break; case 3: LN_FWD(3); break; default: LN_FWD(4); break; }
-#undef LN_FWD
+  const unsigned blocks = grid_for(a->rows, 8, 8);
+  with_nv((int)((a->D + 255) / 256), [&](auto NV) {
+    layernorm_fwd_kernel<NV><<<blocks, 256, 0, s>>>((const bf16*)a->x, (const bf16*)a->gamma, (const bf16*)a->beta, (bf16*)a->y,
+                                                     a->mean, a->rstd, a->rows, (int)a->D, a->ldx, a->ldy, a->eps);
+  });
   DVLA_CHECK_LAUNCH("layernorm_fwd");
   return DVLA_OK;
 }
@@ -516,27 +489,30 @@ extern "C" int dvla_layernorm_bwd(const dvla_layernorm_bwd_args* a, void* stream
   }
   if (a->rows <= 0) return DVLA_OK;
   const int nv = (int)((a->D + 255) / 256);
-  long long blocks = (a->rows + 7) / 8;
+  const unsigned blocks = grid_for(a->rows, 8, 2);   // 2 resident blocks per SM; 2*D fp32 atomics per block at the end
   if (a->D % 256 == 0 && (a->dgamma || a->dbeta) && a->rows >= 2048) {
-    const long long cap3 = 2LL * num_sms();
-    if (blocks > cap3) blocks = cap3;
-    const size_t smem = (size_t)8 * 2 * a->D * sizeof(float);
-#define LN_BWD2(NV) do { \
-      static const cudaError_t attr_e = cudaFuncSetAttribute(layernorm_bwd_v2_kernel<NV>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * 2 * NV * 256 * 4); \
-      if (attr_e != cudaSuccess) { set_error("layernorm_bwd_v2 smem attr: %s", cudaGetErrorString(attr_e)); return DVLA_ERR_CUDA; } \
-      layernorm_bwd_v2_kernel<NV><<<(unsigned)blocks, 256, smem, s>>>((const bf16*)a->dy, (const bf16*)a->x, (const bf16*)a->gamma, \
-          a->mean, a->rstd, (bf16*)a->dx, a->dgamma, a->dbeta, a->rows, a->ld, (const bf16*)a->dres); } while (0)
-    switch (nv) { case 1: LN_BWD2(1); break; case 2: LN_BWD2(2); break; case 3: LN_BWD2(3); break; default: LN_BWD2(4); break; }
-#undef LN_BWD2
+    const int rc = with_nv(nv, [&](auto NV) {
+      constexpr int smem = 8 * 2 * NV * 256 * sizeof(float);
+      static std::once_flag once;
+      static cudaError_t attr_err;
+      if (!set_smem_attr_once(once, attr_err, layernorm_bwd_v2_kernel<NV>, smem)) {
+        set_error("layernorm_bwd_v2 smem attr: %s", cudaGetErrorString(attr_err));
+        return DVLA_ERR_CUDA;
+      }
+      layernorm_bwd_v2_kernel<NV><<<blocks, 256, smem, s>>>((const bf16*)a->dy, (const bf16*)a->x, (const bf16*)a->gamma, a->mean,
+                                                            a->rstd, (bf16*)a->dx, a->dgamma, a->dbeta, a->rows, a->ld,
+                                                            (const bf16*)a->dres);
+      return DVLA_OK;
+    });
+    if (rc != DVLA_OK) return rc;
     DVLA_CHECK_LAUNCH("layernorm_bwd_v2");
     return DVLA_OK;
   }
-  const long long cap = 2LL * num_sms();        // 2 resident blocks per SM; 2*D fp32 atomics per block at the end
-  if (blocks > cap) blocks = cap;
-#define LN_BWD(NV) layernorm_bwd_kernel<NV><<<(unsigned)blocks, 256, 0, s>>>((const bf16*)a->dy, (const bf16*)a->x, \
-      (const bf16*)a->gamma, a->mean, a->rstd, (bf16*)a->dx, a->dgamma, a->dbeta, a->rows, (int)a->D, a->ld, (const bf16*)a->dres)
-  switch (nv) { case 1: LN_BWD(1); break; case 2: LN_BWD(2); break; case 3: LN_BWD(3); break; default: LN_BWD(4); break; }
-#undef LN_BWD
+  with_nv(nv, [&](auto NV) {
+    layernorm_bwd_kernel<NV><<<blocks, 256, 0, s>>>((const bf16*)a->dy, (const bf16*)a->x, (const bf16*)a->gamma, a->mean, a->rstd,
+                                                     (bf16*)a->dx, a->dgamma, a->dbeta, a->rows, (int)a->D, a->ld,
+                                                     (const bf16*)a->dres);
+  });
   DVLA_CHECK_LAUNCH("layernorm_bwd");
   return DVLA_OK;
 }
@@ -545,14 +521,10 @@ extern "C" int dvla_colsum_accum(const void* x, int64_t rows, int64_t N, int64_t
   const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (!x || !out) { set_error("colsum: null pointer"); return DVLA_ERR_INVALID; }
   if (rows <= 0 || N <= 0) return DVLA_OK;
-  const int vec = (N % 8 == 0) && (ld % 8 == 0) && ((reinterpret_cast<uintptr_t>(x) & 15) == 0);
-  const int bx = (int)((N + 255) / 256);
-  int by = (int)((6LL * num_sms() + bx - 1) / bx);     // ~6 blocks of 256 threads per SM: enough loads in flight for HBM
-  if (by > (rows + 63) / 64) by = (int)((rows + 63) / 64);
-  if (by < 1) by = 1;
-  const int rpb = (int)((rows + by - 1) / by);
-  by = (int)((rows + rpb - 1) / rpb);
-  colsum_kernel<<<dim3(bx, by), 256, 0, s>>>((const bf16*)x, rows, (int)N, ld, out, rpb, vec);
+  const int vec = (N % 8 == 0) && (ld % 8 == 0) && aligned16(x);
+  int rpb;
+  const dim3 grid = slab_grid(rows, N, 6, 64, &rpb);    // ~6 blocks of 256 threads per SM: enough loads in flight for HBM
+  colsum_kernel<<<grid, 256, 0, s>>>((const bf16*)x, rows, (int)N, ld, out, rpb, vec);
   DVLA_CHECK_LAUNCH("colsum");
   return DVLA_OK;
 }
@@ -561,9 +533,7 @@ extern "C" int dvla_accum_fp32_into_bf16(const float* src, void* dst, int64_t n,
   const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (!src || !dst) { set_error("accum_fp32_into_bf16: null pointer"); return DVLA_ERR_INVALID; }
   if (n <= 0) return DVLA_OK;
-  long long blocks = (n + 255) / 256;
-  if (blocks > 4LL * num_sms()) blocks = 4LL * num_sms();
-  accum_fp32_into_bf16_kernel<<<(unsigned)blocks, 256, 0, s>>>(src, (bf16*)dst, n);
+  accum_fp32_into_bf16_kernel<<<grid_for(n, 256, 4), 256, 0, s>>>(src, (bf16*)dst, n);
   DVLA_CHECK_LAUNCH("accum_fp32_into_bf16");
   return DVLA_OK;
 }
@@ -577,12 +547,8 @@ extern "C" int dvla_dropout(const void* x, void* y, int64_t rows, int64_t N, int
   uint32_t thresh;
   float scale;
   dropout_thresh_scale(p, &thresh, &scale);
-  const int vec = (N % 8 == 0) && (ldx % 8 == 0) && (ldy % 8 == 0) && ((reinterpret_cast<uintptr_t>(x) & 15) == 0) &&
-                  ((reinterpret_cast<uintptr_t>(y) & 15) == 0);
-  const long long total = rows * ((N + 7) / 8);
-  long long blocks = (total + 255) / 256;
-  if (blocks > 8LL * num_sms()) blocks = 8LL * num_sms();
-  dropout_kernel<<<(unsigned)blocks, 256, 0, s>>>((const bf16*)x, (bf16*)y, rows, (int)N, ldx, ldy, thresh, scale, seed, seed_ptr, vec);
+  const int vec = (N % 8 == 0) && (ldx % 8 == 0) && (ldy % 8 == 0) && aligned16(x, y);
+  dropout_kernel<<<grid_for(rows * ((N + 7) / 8), 256, 8), 256, 0, s>>>((const bf16*)x, (bf16*)y, rows, (int)N, ldx, ldy, thresh, scale, seed, seed_ptr, vec);
   DVLA_CHECK_LAUNCH("dropout");
   return DVLA_OK;
 }
@@ -591,11 +557,10 @@ extern "C" int dvla_act_bwd(const void* dy, const void* pre, void* dx, int64_t n
   const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (!dy || !pre || !dx) { set_error("act_bwd: null pointer"); return DVLA_ERR_INVALID; }
   if (n <= 0) return DVLA_OK;
-  const bool vec = ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(pre) | reinterpret_cast<uintptr_t>(dx)) & 15) == 0;
-  long long blocks = ((vec ? (n + 7) / 8 : n) + 255) / 256;
-  if (blocks > 8LL * num_sms()) blocks = 8LL * num_sms();
-  if (vec) act_bwd_kernel<<<(unsigned)blocks, 256, 0, s>>>((const bf16*)dy, (const bf16*)pre, (bf16*)dx, n, act);
-  else     act_bwd_scalar_kernel<<<(unsigned)blocks, 256, 0, s>>>((const bf16*)dy, (const bf16*)pre, (bf16*)dx, n, act);
+  const bool vec = aligned16(dy, pre, dx);
+  const unsigned blocks = grid_for(vec ? (n + 7) / 8 : n, 256, 8);
+  if (vec) act_bwd_kernel<<<blocks, 256, 0, s>>>((const bf16*)dy, (const bf16*)pre, (bf16*)dx, n, act);
+  else     act_bwd_scalar_kernel<<<blocks, 256, 0, s>>>((const bf16*)dy, (const bf16*)pre, (bf16*)dx, n, act);
   DVLA_CHECK_LAUNCH("act_bwd");
   return DVLA_OK;
 }
@@ -605,19 +570,15 @@ extern "C" int dvla_act_bwd_colsum(const void* dy, const void* pre, void* dx, in
   const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (!dy || !pre || !dx || !colsum) { set_error("act_bwd_colsum: null pointer"); return DVLA_ERR_INVALID; }
   if (rows <= 0 || N <= 0) return DVLA_OK;
-  if (N % 8 || ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(pre) | reinterpret_cast<uintptr_t>(dx)) & 15)) {
+  if (N % 8 || !aligned16(dy, pre, dx)) {
     // unaligned / odd width: the two separate passes
     int rc = dvla_act_bwd(dy, pre, dx, rows * N, act, stream);
     if (rc != DVLA_OK) return rc;
     return dvla_colsum_accum(dx, rows, N, N, colsum, stream);
   }
-  const int bx = (int)((N + 255) / 256);
-  int by = (8 * num_sms() + bx - 1) / bx;
-  if (by > (rows + 31) / 32) by = (int)((rows + 31) / 32);
-  if (by < 1) by = 1;
-  const int rpb = (int)((rows + by - 1) / by);
-  by = (int)((rows + rpb - 1) / rpb);
-  act_bwd_colsum_kernel<<<dim3(bx, by), 256, 0, s>>>((const bf16*)dy, (const bf16*)pre, (bf16*)dx, rows, (int)N, colsum, rpb, act);
+  int rpb;
+  const dim3 grid = slab_grid(rows, N, 8, 32, &rpb);
+  act_bwd_colsum_kernel<<<grid, 256, 0, s>>>((const bf16*)dy, (const bf16*)pre, (bf16*)dx, rows, (int)N, colsum, rpb, act);
   DVLA_CHECK_LAUNCH("act_bwd_colsum");
   return DVLA_OK;
 }
@@ -627,14 +588,8 @@ extern "C" int dvla_cat_broadcast(const void* e, const void* m, void* out, int64
   const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (!e || !m || !out) { set_error("cat_broadcast: null pointer"); return DVLA_ERR_INVALID; }
   if (n <= 0 || a < 0 || b <= 0 || C <= 0 || C % 8) { set_error("cat_broadcast: bad dims (C must be a multiple of 8)"); return DVLA_ERR_INVALID; }
-  if ((reinterpret_cast<uintptr_t>(e) | reinterpret_cast<uintptr_t>(m) | reinterpret_cast<uintptr_t>(out)) & 15) {
-    set_error("cat_broadcast: buffers must be 16-byte aligned"); return DVLA_ERR_INVALID;
-  }
-  const long long total = n * (a + b) * (C / 8);
-  long long blocks = (total + 256 * 4 - 1) / (256 * 4);
-  const long long cap = 16LL * num_sms();
-  if (blocks > cap) blocks = cap;
-  cat_broadcast_kernel<<<(unsigned)blocks, 256, 0, s>>>((const uint4*)e, (const uint4*)m, (uint4*)out, n, (int)a, (int)b, (int)(C / 8));
+  if (!aligned16(e, m, out)) { set_error("cat_broadcast: buffers must be 16-byte aligned"); return DVLA_ERR_INVALID; }
+  cat_broadcast_kernel<<<grid_for(n * (a + b) * (C / 8), 256 * 4, 16), 256, 0, s>>>((const uint4*)e, (const uint4*)m, (uint4*)out, n, (int)a, (int)b, (int)(C / 8));
   DVLA_CHECK_LAUNCH("cat_broadcast");
   return DVLA_OK;
 }
