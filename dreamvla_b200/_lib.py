@@ -50,7 +50,7 @@ class AttnFwdArgs(C.Structure):
                 ("q_sb", _i64), ("q_ss", _i64), ("q_sh", _i64), ("k_sb", _i64), ("k_ss", _i64), ("k_sh", _i64),
                 ("v_sb", _i64), ("v_ss", _i64), ("v_sh", _i64), ("o_sb", _i64), ("o_ss", _i64), ("o_sh", _i64),
                 ("mask_words", _i32), ("scale", _f32), ("dropout_p", _f32), ("dropout_seed", _u64), ("dropout_seed_ptr", _vp),
-                ("key_bias", _vp), ("head_dim", _i64)]
+                ("key_bias", _vp), ("head_dim", _i64), ("mask_index", _vp), ("mask_stride", _i64), ("flags_stride", _i64)]
 
 
 class AttnBwdArgs(C.Structure):
@@ -287,9 +287,11 @@ def _bsh(t, hd=64):
 
 
 def attn_fwd(q, k, v, scale, mask_bits=None, tile_flags=None, dropout_p=0.0, dropout_seed=0, need_lse=True,
-             dropout_seed_ptr=None, key_bias=None):
+             dropout_seed_ptr=None, key_bias=None, mask_index=None):
     """q [B,Lq,H,hd], k/v [B,Lk,H,hd] (arbitrary batch/seq/head strides) -> o [B,Lq,H,hd] contiguous, lse [B,H,Lq].
-    hd = 64, or 96 where the short-sequence kernels run (the library refuses other cases)."""
+    hd = 64, or 96 where the short-sequence kernels run (the library refuses other cases).
+    mask_index: device int32 [B] selecting, per batch, one matrix of the stacks mask_bits [n, Lq, words] / tile_flags
+    [n, nqt, nkt] (contiguous)."""
     _need_cuda(q, k, v)
     B, Lq, H, hd = q.shape
     Lk = k.shape[1]
@@ -303,9 +305,13 @@ def attn_fwd(q, k, v, scale, mask_bits=None, tile_flags=None, dropout_p=0.0, dro
     a.k_sb, a.k_ss, a.k_sh = _bsh(k, hd)
     a.v_sb, a.v_ss, a.v_sh = _bsh(v, hd)
     a.o_sb, a.o_ss, a.o_sh = _bsh(o, hd)
-    a.mask_words = 0 if mask_bits is None else mask_bits.shape[1]
+    a.mask_words = 0 if mask_bits is None else mask_bits.shape[-1]
     a.scale, a.dropout_p, a.dropout_seed = float(scale), float(dropout_p), int(dropout_seed)
     a.dropout_seed_ptr = _ptr(dropout_seed_ptr)
+    if mask_index is not None:
+        assert mask_index.dtype == torch.int32 and mask_index.is_contiguous() and mask_index.numel() == B
+        assert mask_bits.dim() == 3 and mask_bits.is_contiguous() and tile_flags.dim() == 3 and tile_flags.is_contiguous()
+        a.mask_index, a.mask_stride, a.flags_stride = mask_index.data_ptr(), mask_bits[0].numel(), tile_flags[0].numel()
     if key_bias is not None:
         assert key_bias.dtype == torch.float32 and key_bias.is_contiguous() and key_bias.numel() == Lk
         a.key_bias = key_bias.data_ptr()

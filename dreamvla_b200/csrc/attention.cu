@@ -39,6 +39,8 @@ struct AttnParams {
   long long do_sb, do_ss, do_sh, dq_sb, dq_ss, dq_sh, dk_sb, dk_ss, dk_sh, dv_sb, dv_ss, dv_sh;
   float scale;
   float drop_scale; uint32_t drop_thresh; uint64_t drop_seed; const uint64_t* drop_seed_ptr;
+  // forward with per-sequence masks (PER_SEQ kernels): batch b reads mask / tile_flags advanced by mask_index[b] strides
+  const int32_t* mask_index; long long mask_stride, flags_stride;
 };
 
 // ---- smem tile helpers: 64 rows x 64 bf16 (128 B per row), 16-byte chunk c of row r stored at chunk c ^ (r & 7) --------
@@ -190,7 +192,9 @@ __device__ __forceinline__ void dropout_bits(const AttnParams& p, long long bh, 
 // fwd_tile_step, it made the wgmma forward ~1.5% slower at the ViT shape on an H100).
 
 // Mask words of the query rows row0 + lane/4 + {0, 8} over keys [k0, k0 + 64): all ones unless the tile is partial (flag 1).
-__device__ __forceinline__ void row_mask_words(const AttnParams& p, int row0, int k0, int flag, uint32_t (&w)[2][2]) {
+// `mask` is p.mask, or the batch's matrix of a per-sequence stack.
+__device__ __forceinline__ void row_mask_words(const AttnParams& p, const uint32_t* mask, int row0, int k0, int flag,
+                                               uint32_t (&w)[2][2]) {
   const int g = (threadIdx.x & 31) >> 2;
   w[0][0] = w[0][1] = w[1][0] = w[1][1] = 0xffffffffu;
   if (flag != 1) return;
@@ -200,7 +204,7 @@ __device__ __forceinline__ void row_mask_words(const AttnParams& p, int row0, in
 #pragma unroll
     for (int ww = 0; ww < 2; ++ww) {
       const int wi = (k0 >> 5) + ww;
-      w[r][ww] = (row < p.Lq && wi < p.mask_words) ? p.mask[static_cast<long long>(row) * p.mask_words + wi] : 0u;
+      w[r][ww] = (row < p.Lq && wi < p.mask_words) ? mask[static_cast<long long>(row) * p.mask_words + wi] : 0u;
     }
   }
 }
@@ -208,12 +212,13 @@ __device__ __forceinline__ void row_mask_words(const AttnParams& p, int row0, in
 // Forward step over the key tile [k0, k0 + 64) on S = Q K^T (rows = queries from row0): hide the keys the mask (flag 1) or
 // the sequence end hides, scale by sc into the log2 domain, fold the tile into the online softmax (m_run, l_run, o
 // rescaled) and drop elements of P.  Leaves P in s.
-__device__ __forceinline__ void fwd_tile_step(const AttnParams& p, float sc, long long bh, int row0, int k0, int flag,
-                                              float (&s)[8][4], float (&o)[8][4], float (&m_run)[2], float (&l_run)[2]) {
+__device__ __forceinline__ void fwd_tile_step(const AttnParams& p, const uint32_t* mask, float sc, long long bh, int row0,
+                                              int k0, int flag, float (&s)[8][4], float (&o)[8][4], float (&m_run)[2],
+                                              float (&l_run)[2]) {
   const int c = threadIdx.x & 3;
   const bool tail = (k0 + 64 > p.Lk);
   uint32_t w[2][2];
-  row_mask_words(p, row0, k0, flag, w);
+  row_mask_words(p, mask, row0, k0, flag, w);
   float tmax[2] = {-INFINITY, -INFINITY};
 #pragma unroll
   for (int t = 0; t < 8; ++t) {
@@ -277,7 +282,7 @@ __device__ __forceinline__ void dq_form_ds(const AttnParams& p, float sc, long l
                                            const float (&dp)[8][4]) {
   const int c = threadIdx.x & 3;
   uint32_t w[2][2];
-  row_mask_words(p, row0, k0, flag, w);
+  row_mask_words(p, p.mask, row0, k0, flag, w);
   uint32_t keep[8];
   if (p.drop_scale != 0.f) dropout_bits(p, bh, row0, k0, false, keep);
 #pragma unroll
@@ -311,7 +316,20 @@ __device__ __forceinline__ void store_frag_bf16(bf16* dst, long long ss, int row
   }
 }
 
+// Batch b's bit matrix and tile flags: p.mask / p.tile_flags, or (PER_SEQ) the stack entry mask_index[b] selects.
+template <bool PER_SEQ>
+__device__ __forceinline__ void batch_mask(const AttnParams& p, int b, const uint32_t*& mask, const uint8_t*& tile_flags) {
+  mask = p.mask;
+  tile_flags = p.tile_flags;
+  if constexpr (PER_SEQ) {
+    const long long mi = __ldg(p.mask_index + b);
+    mask += mi * p.mask_stride;
+    tile_flags += mi * p.flags_stride;
+  }
+}
+
 // ===================================================== forward ====================================================
+template <bool PER_SEQ>
 __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnParams p) {
   __shared__ __align__(1024) uint8_t sm[5 * 8192];
   const uint32_t sQ = smem_u32(sm), sK0 = sQ + 8192, sV0 = sQ + 2 * 8192, sK1 = sQ + 3 * 8192, sV1 = sQ + 4 * 8192;
@@ -321,7 +339,10 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnParams p) {
   const bf16* qg = p.q + b * p.q_sb + h * p.q_sh;
   const bf16* kg = p.k + b * p.k_sb + h * p.k_sh;
   const bf16* vg = p.v + b * p.v_sb + h * p.v_sh;
-  const uint8_t* flags = p.tile_flags ? p.tile_flags + static_cast<long long>(qt) * p.nkt : nullptr;
+  const uint32_t* mask;
+  const uint8_t* tile_flags;
+  batch_mask<PER_SEQ>(p, b, mask, tile_flags);
+  const uint8_t* flags = tile_flags ? tile_flags + static_cast<long long>(qt) * p.nkt : nullptr;
 
   auto next_tile = [&](int kt) {
     while (kt < p.nkt && flags && flags[kt] == 0) ++kt;
@@ -361,7 +382,7 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnParams p) {
     float s[8][4];
     zero_c(s);
     mma_a_tT(s, qf, sK);
-    fwd_tile_step(p, sc, bh, q0 + warp * 16, kt * 64, flags ? flags[kt] : 2, s, o, m_run, l_run);
+    fwd_tile_step(p, PER_SEQ ? mask : p.mask, sc, bh, q0 + warp * 16, kt * 64, flags ? flags[kt] : 2, s, o, m_run, l_run);
     uint32_t pa[4][4];
     c_to_a(s, pa);
     mma_p_t(o, pa, sV);
@@ -414,6 +435,7 @@ __device__ __forceinline__ void tma_rows(uint32_t dst, const CUtensorMap* m, uin
 
 struct WgmmaFwdMaps { CUtensorMap q, k, v; int q_head_inner, k_head_inner, v_head_inner; };
 
+template <bool PER_SEQ>
 __global__ void __launch_bounds__(WF_THREADS, 2) attn_fwd_wgmma_kernel(const __grid_constant__ WgmmaFwdMaps tm, const AttnParams p) {
   extern __shared__ uint8_t wf_smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(wf_smem_raw) + 1023) & ~uintptr_t(1023));
@@ -428,7 +450,10 @@ __global__ void __launch_bounds__(WF_THREADS, 2) attn_fwd_wgmma_kernel(const __g
   // late query blocks see the most keys under block-causal masks; blockIdx.z is the slowest launch dimension, so every
   // (b, h) starts its heavy blocks before any light one
   const int qt_base = 2 * (static_cast<int>(gridDim.z) - 1 - static_cast<int>(blockIdx.z));
-  const uint8_t* fl0 = p.tile_flags ? p.tile_flags + static_cast<long long>(qt_base) * p.nkt : nullptr;
+  const uint32_t* mask;
+  const uint8_t* tile_flags;
+  batch_mask<PER_SEQ>(p, b, mask, tile_flags);
+  const uint8_t* fl0 = tile_flags ? tile_flags + static_cast<long long>(qt_base) * p.nkt : nullptr;
   const bool has1 = qt_base + 1 < p.nqt;
   auto needed = [&](int kt, int g) -> bool {   // does q-tile qt_base+g see any key of k-tile kt?
     if (g == 1 && !has1) return false;
@@ -492,7 +517,7 @@ __global__ void __launch_bounds__(WF_THREADS, 2) attn_fwd_wgmma_kernel(const __g
       wgmma_commit();
       wgmma_wait<0>();
       wgmma_fence_operand32(sd);
-      fwd_tile_step(p, sc, bh, q0 + wq * 16, kt * 64, flag, s, o, m_run, l_run);
+      fwd_tile_step(p, PER_SEQ ? mask : p.mask, sc, bh, q0 + wq * 16, kt * 64, flag, s, o, m_run, l_run);
       uint32_t pa[4][4];
       c_to_a(s, pa);
       float (&od)[32] = *reinterpret_cast<float(*)[32]>(&o[0][0]);
@@ -994,6 +1019,7 @@ static bool tmap_strides_ok(long long L, long long H, long long B, long long ss,
   return (sh < ss) ? (sh >= 64 && ss >= sh * H) : (ss >= 64 && sh >= ss * L);
 }
 
+template <bool PER_SEQ>
 static int attn_fwd_wgmma_launch(const dvla_attn_fwd_args* a, const AttnParams& p, cudaStream_t s) {
   WgmmaFwdMaps tm;
   if (!make_attn_tmap(&tm.q, a->q, a->Lq, a->H, a->B, a->q_ss, a->q_sh, a->q_sb, &tm.q_head_inner) ||
@@ -1002,8 +1028,8 @@ static int attn_fwd_wgmma_launch(const dvla_attn_fwd_args* a, const AttnParams& 
     return DVLA_ERR_CUDA;
   static std::once_flag once;
   static cudaError_t attr_err = cudaSuccess;
-  if (!set_smem_attr_once(once, attr_err, attn_fwd_wgmma_kernel, WF_SMEM)) { set_error("attn_fwd_wgmma smem attribute: %s", cudaGetErrorString(attr_err)); return DVLA_ERR_CUDA; }
-  attn_fwd_wgmma_kernel<<<dim3(p.H, p.B, (p.nqt + 1) / 2), WF_THREADS, WF_SMEM, s>>>(tm, p);
+  if (!set_smem_attr_once(once, attr_err, attn_fwd_wgmma_kernel<PER_SEQ>, WF_SMEM)) { set_error("attn_fwd_wgmma smem attribute: %s", cudaGetErrorString(attr_err)); return DVLA_ERR_CUDA; }
+  attn_fwd_wgmma_kernel<PER_SEQ><<<dim3(p.H, p.B, (p.nqt + 1) / 2), WF_THREADS, WF_SMEM, s>>>(tm, p);
   DVLA_CHECK_LAUNCH("attn_fwd_wgmma");
   return DVLA_OK;
 }
@@ -1058,19 +1084,30 @@ extern "C" int dvla_attn_fwd(const dvla_attn_fwd_args* a, void* stream) {
   if (!dropout_rate_ok(a->dropout_p)) { set_error("attn_fwd: dropout_p out of range [0, 1)"); return DVLA_ERR_INVALID; }
   const bool small = attn_small_applicable(a->Lq, a->Lk, a->mask, a->dropout_p);
   if (!head_dim_ok(a->head_dim, small)) return head_dim_unsupported("attn_fwd", a);
-  if (small) return attn_small_fwd(a, s);
-  if (a->key_bias) {
+  // (the short-sequence kernels take no mask, so there a mask_index always lacks one)
+  const bool index_without_mask = a->mask_index && !a->mask;
+  if (small && !index_without_mask) return attn_small_fwd(a, s);
+  if (a->key_bias && !small) {
     set_error("attn_fwd: key_bias needs the short-sequence kernels (Lq <= 32, Lk <= 64, no mask, no dropout)");
     return DVLA_ERR_UNSUPPORTED;
   }
+  if (index_without_mask) { set_error("attn_fwd: mask_index given without mask"); return DVLA_ERR_INVALID; }
+  if (a->mask_index && (a->mask_stride < 0 || a->flags_stride < 0)) {
+    set_error("attn_fwd: negative mask_stride %lld / flags_stride %lld", (long long)a->mask_stride, (long long)a->flags_stride);
+    return DVLA_ERR_INVALID;
+  }
   AttnParams p = attn_params(a);
   p.out = (bf16*)a->o;
+  // a mask implies the kernels below (the short-sequence ones take none), and each has a per-sequence-mask variant
+  const bool per_seq = a->mask_index != nullptr;
+  p.mask_index = a->mask_index; p.mask_stride = a->mask_stride; p.flags_stride = a->flags_stride;
   // wgmma + TMA for the long sequences (backbone, ViT, decoders); the mma.sync kernel for short query blocks and strides a
   // tensor map cannot express
   if (a->Lq >= 96 && tmap_strides_ok(a->Lq, a->H, a->B, a->q_ss, a->q_sh, a->q_sb) &&
       tmap_strides_ok(a->Lk, a->H, a->B, a->k_ss, a->k_sh, a->k_sb) && tmap_strides_ok(a->Lk, a->H, a->B, a->v_ss, a->v_sh, a->v_sb))
-    return attn_fwd_wgmma_launch(a, p, s);
-  attn_fwd_kernel<<<dim3(p.nqt, p.H, p.B), 128, 0, s>>>(p);
+    return per_seq ? attn_fwd_wgmma_launch<true>(a, p, s) : attn_fwd_wgmma_launch<false>(a, p, s);
+  if (per_seq) attn_fwd_kernel<true><<<dim3(p.nqt, p.H, p.B), 128, 0, s>>>(p);
+  else         attn_fwd_kernel<false><<<dim3(p.nqt, p.H, p.B), 128, 0, s>>>(p);
   DVLA_CHECK_LAUNCH("attn_fwd");
   return DVLA_OK;
 }

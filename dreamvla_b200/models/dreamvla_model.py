@@ -69,6 +69,45 @@ def generate_attention_mask(K, num_A, num_B, atten_goal, atten_goal_state, atten
     return mask
 
 
+def prune_closure(vis, sel, n_tok):
+    """Token indices (ascending) a rollout keeps for timestep `sel` under the visibility matrix vis [L, L] (bool): every slot
+    of timestep sel plus, transitively, every slot a kept row can see."""
+    keep = torch.zeros(vis.shape[0], dtype=torch.bool)
+    keep[sel * n_tok:(sel + 1) * n_tok] = True               # every slot of the selected timestep
+    while True:                                              # + everything a kept row can see (transitively)
+        grown = keep | vis[keep].any(dim=0)
+        if bool((grown == keep).all()):
+            return keep.nonzero().flatten()
+        keep = grown
+
+
+def batched_rollout_layout(vis, S, n_a, action_pred_steps):
+    """Per timestep sel of a window of S: idx_sel = prune_closure(sel) + the A slots (the first n_a of a timestep) of the
+    timesteps after sel, in token order, and the position of sel's first action row in it.  Every idx_sel must have the same
+    length and start with the pruned single-env sequence (then a batch of envs at any mix of sel shares one sequence length,
+    and each env's kept rows compute what they compute alone); ValueError otherwise.  -> (idx [S, Lb] int64, r0 [S] int64)."""
+    n_tok = vis.shape[0] // S
+    rows, r0s = [], []
+    for sel in range(S):
+        kept = prune_closure(vis, sel, n_tok)
+        want = torch.zeros(vis.shape[0], dtype=torch.bool)
+        want[kept] = True
+        for t in range(sel + 1, S):
+            want[t * n_tok:t * n_tok + n_a] = True
+        idx = want.nonzero().flatten()
+        if not torch.equal(idx[:len(kept)], kept):
+            raise ValueError(f"batched rollout: under this attention mask the pruned sequence of timestep {sel} is not a prefix "
+                             "of its batched layout; use rollout_action per env")
+        rows.append(idx)
+        a0 = sel * n_tok + n_tok - action_pred_steps            # first action row of timestep sel
+        r0s.append(int((kept < a0).sum()))
+    lens = sorted({len(r) for r in rows})
+    if len(lens) != 1:
+        raise ValueError(f"batched rollout: the kept-token count differs between timesteps ({lens}) under this attention "
+                         "mask, so the envs cannot share one batch; use rollout_action per env")
+    return torch.stack(rows), torch.tensor(r0s, dtype=torch.long)
+
+
 class _WorldDecoder(nn.Module):
     """Helper that RUNS one world-knowledge decoder (reference :793-911); it owns no parameters -- the parameters stay
     on DreamVLA under the reference names.
@@ -540,9 +579,16 @@ class DreamVLA(nn.Module):
                 and net.x_embedder.linear.weight.shape[0] in (64 * net.num_heads, 96 * net.num_heads)
                 and not torch.is_grad_enabled())
 
-    def _ddim_actions(self, feat, sample_noise, dev):
-        """10-step DDIM with classifier-free guidance 1.5 (:935-987) on feat [n, action_pred_steps, D] -> [n, steps, 7]."""
+    # Most sequences a batched rollout samples on the fused kernel.  The kernel takes up to 8 (its tensor-core bucket,
+    # csrc/dit_sampler.cu), but on an H100 that bucket is slower than the launch-bound module sampler at every N >= 2
+    # (tools/prof_batched_rollout.py, DESIGN §8), so the measured crossover keeps N >= 2 on the module sampler.
+    FUSED_SAMPLER_MAX_BATCH = 1
+
+    def _ddim_actions(self, feat, sample_noise, dev, multi=False):
+        """10-step DDIM with classifier-free guidance 1.5 (:935-987) on feat [n, action_pred_steps, D] -> [n, steps, 7].
+        multi=True (batched rollouts): the fused kernel takes up to FUSED_SAMPLER_MAX_BATCH sequences."""
         bs = feat.shape[0]
+        fused = self._fused_sampler_fits(bs) or (multi and bs <= self.FUSED_SAMPLER_MAX_BATCH and self._fused_sampler_fits(1))
         cfg_scale = 1.5
         if self.use_fm:
             # --use_fm (ActionModelFM / FMDiffusion, respace.py:118-191): the sampler forces the guidance scale to 1.0, ignores
@@ -551,7 +597,7 @@ class DreamVLA(nn.Module):
             if self.action_model.ddim_diffusion is None:
                 self.action_model.create_ddim(ddim_step=10)
             shape = (2 * bs, self.action_pred_steps, self.action_model.in_channels)
-            if self._fused_sampler_fits(bs) and self.action_model.ddim_diffusion.num_timesteps <= 12:
+            if fused and self.action_model.ddim_diffusion.num_timesteps <= 12:
                 # the same start-state draw as FMDiffusion (the CUDA generator advances alike on both paths); the kernel
                 # integrates the first half, the only one that reaches the output
                 start = sample_noise if sample_noise is not None else torch.randn(*shape, device=dev)
@@ -576,8 +622,8 @@ class DreamVLA(nn.Module):
         if self.action_model.ddim_diffusion is None:
             self.action_model.create_ddim(ddim_step=10)
         net = self.action_model.net
-        if self._fused_sampler_fits(bs):
-            # one sequence (rollouts): the whole guided DDIM loop as one persistent kernel (csrc/dit_sampler.cu)
+        if fused:
+            # rollouts: the whole guided DDIM loop as one persistent kernel (csrc/dit_sampler.cu)
             from .. import _lib as L
             return L.dit_ddim_sample(net, self.action_model.ddim_diffusion, feat.to(torch.bfloat16), noise[:bs].float(),
                                      cfg_scale).to(feat.dtype)
@@ -615,17 +661,59 @@ class DreamVLA(nn.Module):
         if key not in cache:
             n_tok = self.attention_mask.shape[0] // self.sequence_length
             vis = (self.attention_mask.detach().float().cpu() == 0)
-            keep = torch.zeros(vis.shape[0], dtype=torch.bool)
-            keep[sel * n_tok:(sel + 1) * n_tok] = True               # every slot of the selected timestep
-            while True:                                              # + everything a kept row can see (transitively)
-                grown = keep | vis[keep].any(dim=0)
-                if bool((grown == keep).all()):
-                    break
-                keep = grown
-            idx = keep.nonzero().flatten()
+            idx = prune_closure(vis, sel, n_tok)
             cache[key] = (ops.AttnMask.from_additive(self.attention_mask.detach().float().cpu()[idx][:, idx].contiguous(),
                                                      device), idx.to(device), idx)
         return cache[key]
+
+    def _batched_rollout_tables(self, device):
+        """`batched_rollout_layout` of the model's mask, built on the host once per mask and device -> (AttnMaskStack of the S
+        masks M[idx_sel][:, idx_sel], idx [S, Lb], first action row [S]) on the device.  For the finetune / evaluate masks
+        idx_sel is A slots 0..sel, B slots of sel, A slots sel+1..S-1 (36*S + n_B tokens for every sel); no kept row sees the
+        appended A slots (:41)."""
+        key = (self.attention_mask.data_ptr(), self.attention_mask._version, str(device))
+        cache = self.__dict__.setdefault("_batched_rollout_cache", {})
+        if key not in cache:
+            vis = self.attention_mask.detach().float().cpu() == 0
+            idx, r0 = batched_rollout_layout(vis, self.sequence_length, 1 + 1 + 2 * self.NUM_RESAMPLER_QUERY + 2,
+                                             self.action_pred_steps)
+            stack = ops.AttnMaskStack(torch.stack([vis[r][:, r] for r in idx]), device)
+            cache[key] = (stack, idx.to(device), r0.to(device))
+        return cache[key]
+
+    @torch.no_grad()
+    def rollout_actions(self, text_embedding, frame_tokens, sel, sample_noise=None, return_features=False):
+        """`rollout_action(..., sel[e], prune=True)` for N envs in one batch: one backbone pass over N sequences of equal length
+        (`_batched_rollout_tables`), each under its own mask, then one sampler call for the N action-token groups.
+
+        text_embedding [N, D], frame_tokens [N, S, 35, D] (window order), sel int32 [N] on the device: every per-env choice --
+        mask, token gather, action-row gather -- is made on the device, so one CUDA graph serves every mix of fill levels.
+        sample_noise [N, steps, 7] or None.  Returns (arm [N, steps, 6], gripper [N, steps, 1]), or the backbone's action-token
+        rows [N, steps, D] with return_features.  The actions come from the fused sampler kernel up to FUSED_SAMPLER_MAX_BATCH
+        envs (with FUSED_SAMPLER), from the module sampler above (see FUSED_SAMPLER_MAX_BATCH)."""
+        assert self.use_dit_head and self.action_pred_steps > 0
+        N, S = frame_tokens.shape[:2]
+        D = self.hidden_dim
+        dev = frame_tokens.device
+        assert S == self.sequence_length and sel.dtype == torch.int32 and sel.shape == (N,)
+        stack, idx, r0 = self._batched_rollout_tables(dev)
+        q = torch.cat([t.reshape(-1, D) for t in self._query_tokens()], dim=0)                    # [n_b, D]
+        n_b = q.shape[0]
+        n_tok = 1 + frame_tokens.shape[2] + n_b
+        pos = self.transformer_backbone_position_embedding.view(1, S, 1, D)
+        a_tok = torch.cat((text_embedding.view(N, 1, 1, D).expand(N, S, 1, D), frame_tokens), dim=2)   # [N, S, 36, D]
+        full = (torch.cat((a_tok, q.view(1, 1, n_b, D).expand(N, S, n_b, D)), dim=2) + pos).reshape(N * S * n_tok, D)
+        sel64 = sel.long()
+        rows = idx.index_select(0, sel64) + (torch.arange(N, device=dev) * (S * n_tok)).unsqueeze(1)    # [N, Lb]
+        x = full.index_select(0, rows.flatten()).view(N, -1, D)
+        x = self.embedding_layer_norm(x.contiguous())
+        h = self.transformer_backbone(inputs_embeds=x, attention_mask=stack.select(sel))
+        arow = r0.index_select(0, sel64).unsqueeze(1) + torch.arange(self.action_pred_steps, device=dev)  # [N, steps]
+        feat = h.gather(1, arow.unsqueeze(2).expand(N, self.action_pred_steps, D))                 # [N, steps, D]
+        if return_features:
+            return feat
+        samples = self._ddim_actions(feat, sample_noise, dev, multi=True)
+        return samples[..., :6], samples[..., 6:]
 
     @torch.no_grad()
     def rollout_action(self, text_embedding, frame_tokens, sel, sample_noise=None, prune=True, return_features=False):

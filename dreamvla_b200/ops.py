@@ -333,6 +333,42 @@ class AttnMask:
         return AttnMask(torch.ones(n, n, dtype=torch.bool).tril(), device)
 
 
+class AttnMaskStack:
+    """n bit-matrix masks of one shape, stacked (bits [n, Lq, words], flags [n, nqt, nkt]), for batched calls in which every
+    sequence attends under its own mask: `select(index)` names, per batch entry, the mask it uses (device int32 [B]), so the
+    choice can change between CUDA-graph replays without a host read.  Forward only: the attention ops refuse it when autograd
+    would need a backward."""
+
+    def __init__(self, visible_bool: torch.Tensor, device):
+        assert visible_bool.dim() == 3 and visible_bool.dtype == torch.bool
+        self.n, self.Lq, self.Lk = visible_bool.shape
+        self.bits = torch.stack([AttnMask.pack_bits(m) for m in visible_bool]).to(device).contiguous()
+        self.flags = torch.stack([L.attn_mask_tiles(b, self.Lq, self.Lk) for b in self.bits]).contiguous()
+        self.index = None
+
+    def select(self, index: torch.Tensor) -> "AttnMaskStack":
+        """This stack with batch entry b under mask index[b] (int32 [B] on the stack's device; values in [0, n))."""
+        assert index.dtype == torch.int32 and index.dim() == 1 and index.device == self.bits.device
+        sel = object.__new__(AttnMaskStack)
+        sel.__dict__.update(self.__dict__)
+        sel.index = index
+        return sel
+
+
+def _mask_args(mask, q_len, k_len, need_grad):
+    """(bits, flags, index) of an AttnMask / selected AttnMaskStack / None for L.attn_fwd."""
+    if mask is None:
+        return None, None, None
+    assert mask.Lq == q_len and mask.Lk == k_len, "mask shape mismatch"
+    index = getattr(mask, "index", None)
+    if isinstance(mask, AttnMaskStack):
+        if index is None:
+            raise ValueError("AttnMaskStack used without select(index)")
+        if need_grad:
+            raise RuntimeError("per-sequence attention masks (AttnMaskStack) are forward only: run under torch.no_grad()")
+    return mask.bits, mask.flags, index
+
+
 class ObsDropMask(AttnMask):
     """AttnMask redrawn on the device: every draw() hides `count` of each timestep's n_obs observation columns from that
     timestep's action rows (the pretrain phase's per-forward drop, dreamvla_model.py:55-59), writing `bits` and `flags` in
@@ -385,12 +421,10 @@ class _Attention(torch.autograd.Function):
     def forward(ctx, q, k, v, scale, mask, dropout_p, key_bias=None):
         need = _grad_on and any(ctx.needs_input_grad)
         seed = next_seed() if dropout_p > 0 else 0
-        bits = mask.bits if mask is not None else None
-        flags = mask.flags if mask is not None else None
-        if mask is not None:
-            assert mask.Lq == q.shape[1] and mask.Lk == k.shape[1], "mask shape mismatch"
+        bits, flags, index = _mask_args(mask, q.shape[1], k.shape[1], need)
         o, lse = L.attn_fwd(q, k, v, scale, bits, flags, dropout_p, seed, need_lse=need,
-                            dropout_seed_ptr=seed_counter(q.device) if dropout_p > 0 else None, key_bias=key_bias)
+                            dropout_seed_ptr=seed_counter(q.device) if dropout_p > 0 else None, key_bias=key_bias,
+                            mask_index=index)
         if need:
             ctx.save_for_backward(q, k, v, o, lse)
         ctx.meta = (scale, mask, dropout_p, seed, key_bias)
@@ -418,9 +452,10 @@ class _Attention(torch.autograd.Function):
         return dq, dk, dv, None, None, None, None
 
 
-def attention(q, k, v, scale, mask: AttnMask | None = None, dropout_p: float = 0.0, key_bias=None):
+def attention(q, k, v, scale, mask: AttnMask | AttnMaskStack | None = None, dropout_p: float = 0.0, key_bias=None):
     """q [B,Lq,H,hd], k/v [B,Lk,H,hd] (strided views allowed) -> [B,Lq,H,hd] contiguous.  hd = 64, or 96 on short
-    sequences (Lq <= 32, Lk <= 64, no mask, no dropout).
+    sequences (Lq <= 32, Lk <= 64, no mask, no dropout).  mask: one mask for every batch entry, or a selected
+    AttnMaskStack (a mask per batch entry, forward only).
     key_bias: optional fp32 [Lk] added to the scaled scores (log r = key counted r times); short sequences only."""
     return _apply(_Attention, q, k, v, float(scale), mask, float(dropout_p), key_bias)
 
@@ -433,9 +468,9 @@ class _FusedQKVAttention(torch.autograd.Function):
         need = _grad_on and any(ctx.needs_input_grad)
         seed = next_seed() if dropout_p > 0 else 0
         q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
-        o, lse = L.attn_fwd(q, k, v, scale, mask.bits if mask is not None else None,
-                            mask.flags if mask is not None else None, dropout_p, seed, need_lse=need,
-                            dropout_seed_ptr=seed_counter(qkv.device) if dropout_p > 0 else None)
+        bits, flags, index = _mask_args(mask, q.shape[1], k.shape[1], need)
+        o, lse = L.attn_fwd(q, k, v, scale, bits, flags, dropout_p, seed, need_lse=need,
+                            dropout_seed_ptr=seed_counter(qkv.device) if dropout_p > 0 else None, mask_index=index)
         if need:
             ctx.save_for_backward(qkv, o, lse)
         ctx.meta = (scale, mask, dropout_p, seed)
@@ -453,7 +488,7 @@ class _FusedQKVAttention(torch.autograd.Function):
         return dqkv, None, None, None
 
 
-def self_attention_fused(qkv, scale, mask: AttnMask | None = None, dropout_p: float = 0.0):
+def self_attention_fused(qkv, scale, mask: AttnMask | AttnMaskStack | None = None, dropout_p: float = 0.0):
     """qkv [B, L, 3, H, hd] contiguous bf16 -> [B, L, H, hd]; hd = 64, or 96 on short sequences (see `attention`)."""
     assert qkv.dim() == 5 and qkv.shape[2] == 3 and qkv.shape[4] in (64, 96) and qkv.is_contiguous()
     return _apply(_FusedQKVAttention, qkv, float(scale), mask, float(dropout_p))

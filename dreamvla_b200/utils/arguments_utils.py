@@ -60,7 +60,7 @@ _FLAGS = [
 # --exchange_on_boundary_only: with gradient accumulation, all-reduce + clip once per optimiser step instead of the
 # reference's every-micro-step exchange and in-place clip (utils/train_utils.py:599-600); a different update, opt-in.
 _EXTRA = [("--synthetic_steps", int, 0), ("--cuda_graph", "flag", False), ("--synthetic_rollout_steps", int, 0),
-          ("--exchange_on_boundary_only", "flag", False), ("--incremental_rollout", "flag", False),
+          ("--exchange_on_boundary_only", "flag", False), ("--incremental_rollout", "flag", False), ("--num_envs", int, 1),
           ("--device_augment", "flag", False)]
 
 

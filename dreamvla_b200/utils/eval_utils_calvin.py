@@ -159,14 +159,15 @@ class RolloutEngine:
     def _frame(self, image, flip_vertical=False):
         """-> [1, 1, 3, 224, 224] in the cast dtype on the device.  A raw uint8 [h, w, 3] frame (numpy array or tensor, as the
         simulator returns it) is uploaded as bytes and put through CLIP's image transform on the device (`preprocess_image`,
-        the reference's `image_process_fn`, :82-90); a preprocessed [3, 224, 224] tensor is only moved and cast."""
+        the reference's `image_process_fn`, :82-90); a preprocessed [3, 224, 224] tensor is only moved and cast.  A stack of
+        n frames ([n, h, w, 3] / [n, 3, 224, 224]) gives [n, 1, 3, 224, 224] the same way, in one call."""
         if isinstance(image, np.ndarray):
             image = torch.from_numpy(np.ascontiguousarray(image))
         if image.dtype != torch.uint8:
-            return image.to(self.device, self.cast_type).view(1, 1, 3, 224, 224)
+            return image.to(self.device, self.cast_type).view(-1, 1, 3, 224, 224)
         out_dtype = self.cast_type if self.cast_type in (torch.float32, torch.bfloat16) else torch.float32
         x = preprocess_image(image.to(self.device), out_dtype, flip_vertical)
-        return x.to(self.cast_type).view(1, 1, 3, 224, 224)
+        return x.to(self.cast_type).view(-1, 1, 3, 224, 224)
 
     @torch.no_grad()
     def infer(self, image_static, image_gripper, state_vec, text_tokens, sample_noise=None, flip_static=False):
@@ -218,4 +219,175 @@ class ModelWrapper(RolloutEngine):
         arm, gripper, _ = self.infer(image_static, image_gripper, st, text_tokens, sample_noise)
         action = torch.cat((arm[0].float(), (gripper[0] > 0.5).float()), dim=-1)    # first of the predicted steps (:138)
         action[-1] = (action[-1] - 0.5) * 2                                # scale to -1 or 1 (:139)
+        return action.to(torch.float16).cpu().numpy()
+
+
+class BatchedRolloutEngine(RolloutEngine):
+    """`num_envs` rollouts served by one model: one step call takes the observations of any subset of the envs and runs one
+    batched encode + one batched action inference for all of them, instead of one `RolloutEngine.infer` per env.
+
+    Per env the window semantics are RolloutEngine's: growing then sliding window of `history_len`, padded by repeating the
+    last frame, instruction frozen at the episode's first step, `reset(env)`.  The windows live on the device in window
+    order, for all envs at once: the frame-token windows [N, S, 35, D] (incremental=True, `DreamVLA.rollout_actions`, where
+    each env selects its timestep on the device) or the preprocessed frames [N, S, 3, 224, 224] x 2 and states
+    (incremental=False: a batch-N full-window `mode='test'` forward, the selected row taken per env).  With use_cuda_graph,
+    each of these runs as one CUDA graph over all N envs, replayed whatever the envs' fill levels; envs outside the step
+    are computed and discarded."""
+
+    def __init__(self, model, num_envs, cast_dtype=torch.bfloat16, history_len=10, action_pred_steps=3, device="cuda",
+                 use_cuda_graph=True, incremental=True, state_dim=7):
+        self.num_envs = num_envs
+        super().__init__(model, cast_dtype, history_len, action_pred_steps, device, use_cuda_graph, incremental, True, state_dim)
+        self.fill = [0] * num_envs               # frames pushed since the env's last reset (capped at history_len)
+        self.text_set = [False] * num_envs
+        self._win = None
+
+    def reset_window(self, env=None):
+        if env is None:
+            super().reset_window()
+            return
+        self.fill[env] = 0
+        self.text_set[env] = False
+
+    def _alloc(self, tok_shape, text_dtype):
+        N, S, dev = self.num_envs, self.history_len, self.device
+        steps = self.action_pred_steps
+        w = dict(sel=torch.zeros(N, dtype=torch.int32, device=dev), text_token=torch.zeros(N, 77, dtype=text_dtype, device=dev))
+        if self.incremental:
+            w.update(tok=torch.zeros(N, S, *tok_shape, dtype=self.cast_type, device=dev),
+                     txt=torch.zeros(N, tok_shape[-1], dtype=self.cast_type, device=dev),
+                     p=torch.zeros(N, 3, 224, 224, dtype=self.cast_type, device=dev),
+                     w=torch.zeros(N, 3, 224, 224, dtype=self.cast_type, device=dev),
+                     s=torch.zeros(N, self.state_dim, dtype=self.cast_type, device=dev),
+                     noise=torch.zeros(N, steps, 7, device=dev))
+        else:
+            w.update(img=torch.zeros(N, S, 3, 224, 224, dtype=self.cast_type, device=dev),
+                     grip=torch.zeros(N, S, 3, 224, 224, dtype=self.cast_type, device=dev),
+                     state=torch.zeros(N, S, self.state_dim, dtype=self.cast_type, device=dev),
+                     noise=torch.zeros(N * S, steps, 7, device=dev))
+        self._win = w
+
+    @staticmethod
+    def _push(win, env, n_prev, x):
+        """Append x to the window row win[env] that holds n_prev frames: fill (and pad with x) while growing, slide when full."""
+        S = win.shape[1]
+        if n_prev < S:
+            win[env, n_prev:] = x
+        else:
+            win[env, :-1] = win[env, 1:].clone()
+            win[env, -1] = x
+
+    def _encode_frames(self):
+        st = self._win
+        run = lambda: self.model.encode_frame_tokens(st["p"], st["w"], st["s"])        # noqa: E731
+        if not self.use_cuda_graph:
+            return run()
+        if self._enc_graph is None:
+            self._enc_graph, self._enc_out = self._capture(run)
+        self._enc_graph.replay()
+        return self._enc_out
+
+    def _run_actions(self):
+        st = self._win
+        N, S = self.num_envs, self.history_len
+        if self.incremental:
+            def run():
+                return self.model.rollout_actions(st["txt"], st["tok"], st["sel"], sample_noise=st["noise"])
+        else:
+            def run():
+                out = self.model(image_primary=st["img"], image_wrist=st["grip"], state=st["state"],
+                                 text_token=st["text_token"].unsqueeze(1).expand(N, S, 77), action=None, mode="test",
+                                 sample_noise=st["noise"])
+                rows = torch.arange(N, device=st["sel"].device) * S + st["sel"].long()
+                return out[0][0].index_select(0, rows), out[1][0].index_select(0, rows)
+        if not self.use_cuda_graph:
+            return run()
+        if self._graph is None:
+            self._graph, self._out = self._capture(run)
+        self._graph.replay()
+        return self._out
+
+    @torch.no_grad()
+    def infer_batch(self, envs, image_static, image_gripper, states, text_tokens, sample_noise=None, flip_static=False):
+        """One observation for each env in `envs` (distinct indices < num_envs) -> (arm [n, steps, 6], gripper [n, steps, 1],
+        num_step list) of each env's selected timestep.
+        image_*: stacked [n, h, w, 3] uint8 frames (or a list of them, preprocessed on the device in one call) or preprocessed
+        [n, 3, 224, 224]; states [n, state_dim]; text_tokens int [n, 77] (read at an env's first step after a reset only).
+        sample_noise: [n, steps, 7] start noise of the selected rows, or None (drawn on the device)."""
+        envs = [int(e) for e in envs]
+        n, S, dev = len(envs), self.history_len, self.device
+        assert n and len(set(envs)) == n and all(0 <= e < self.num_envs for e in envs), envs
+
+        def stack(x):
+            if isinstance(x, (list, tuple)):
+                x = [torch.from_numpy(np.ascontiguousarray(f)) if isinstance(f, np.ndarray) else f for f in x]
+                x = torch.stack(x)
+            return torch.from_numpy(np.ascontiguousarray(x)) if isinstance(x, np.ndarray) else x
+        img = self._frame(stack(image_static), flip_static)[:, 0]                          # [n, 3, 224, 224]
+        grip = self._frame(stack(image_gripper))[:, 0]
+        st = torch.as_tensor(stack(states)).to(dev, self.cast_type).view(n, -1)
+        assert st.shape[-1] == self.state_dim, f"state has {st.shape[-1]} dims, the model expects {self.state_dim}"
+        text_tokens = torch.as_tensor(stack(text_tokens)).to(dev).view(n, 77)
+        if self._win is None:
+            tok_shape = None
+            if self.incremental:
+                tok_shape = self.model.encode_frame_tokens(img[:1], grip[:1], st[:1]).shape[1:]
+            self._alloc(tok_shape, text_tokens.dtype)
+        w = self._win
+        idx = torch.tensor(envs, device=dev)
+        new = [i for i, e in enumerate(envs) if not self.text_set[e]]
+        if new:                                                  # frozen for the episode (:110-113)
+            rows = torch.tensor(new, device=dev)
+            w["text_token"].index_copy_(0, idx[rows], text_tokens[rows])
+            if self.incremental:
+                w["txt"].index_copy_(0, idx[rows], self.model.encode_text_embedding(text_tokens[rows]).to(self.cast_type))
+            for i in new:
+                self.text_set[envs[i]] = True
+        if self.incremental:
+            w["p"].index_copy_(0, idx, img)
+            w["w"].index_copy_(0, idx, grip)
+            w["s"].index_copy_(0, idx, st)
+            toks = self._encode_frames().index_select(0, idx)
+        num_steps = []
+        for i, e in enumerate(envs):
+            if self.incremental:
+                self._push(w["tok"], e, self.fill[e], toks[i])
+            else:
+                self._push(w["img"], e, self.fill[e], img[i])
+                self._push(w["grip"], e, self.fill[e], grip[i])
+                self._push(w["state"], e, self.fill[e], st[i])
+            self.fill[e] = min(self.fill[e] + 1, S)
+            num_steps.append(self.fill[e])
+        sel = torch.tensor([max(f - 1, 0) for f in self.fill], dtype=torch.int32)    # == -1 once full (:142-145)
+        w["sel"].copy_(sel)
+        if sample_noise is None:
+            w["noise"].normal_()
+        elif self.incremental:
+            w["noise"].index_copy_(0, idx, sample_noise.to(dev, torch.float32))
+        else:                                                    # the selected row of each env's [S, steps, 7] draw
+            w["noise"].view(self.num_envs, S, *w["noise"].shape[1:])[idx, sel.to(dev).long()[idx]] = \
+                sample_noise.to(dev, torch.float32)
+        arm, gripper = self._run_actions()
+        return arm.index_select(0, idx), gripper.index_select(0, idx), num_steps
+
+
+class BatchedModelWrapper(BatchedRolloutEngine):
+    """CALVIN rollout wrapper for `num_envs` environments: `ModelWrapper.step` per env, batched (see BatchedRolloutEngine)."""
+
+    def __init__(self, model, num_envs, cast_dtype=torch.bfloat16, history_len=10, action_pred_steps=3, device="cuda",
+                 use_cuda_graph=True, incremental=True):
+        super().__init__(model, num_envs, cast_dtype, history_len, action_pred_steps, device, use_cuda_graph, incremental,
+                         state_dim=7)
+
+    def reset(self, env):
+        self.reset_window(env)
+
+    @torch.no_grad()
+    def step(self, envs, image_static, image_gripper, robot_obs, text_tokens, sample_noise=None):
+        """robot_obs [n, 15], text_tokens int [n, 77], images as `infer_batch` takes them -> actions [n, 7] (fp16 numpy)."""
+        obs = torch.as_tensor(np.asarray(robot_obs) if not torch.is_tensor(robot_obs) else robot_obs).reshape(len(envs), -1)
+        st = torch.cat([obs[:, :6], obs[:, -1:]], dim=-1)                  # :104
+        arm, gripper, _ = self.infer_batch(envs, image_static, image_gripper, st, text_tokens, sample_noise)
+        action = torch.cat((arm[:, 0].float(), (gripper[:, 0] > 0.5).float()), dim=-1)   # first of the predicted steps (:138)
+        action[:, -1] = (action[:, -1] - 0.5) * 2                          # scale to -1 or 1 (:139)
         return action.to(torch.float16).cpu().numpy()

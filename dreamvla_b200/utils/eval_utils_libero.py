@@ -16,7 +16,7 @@ from __future__ import annotations
 import numpy as np
 import torch
 
-from .eval_utils_calvin import RolloutEngine
+from .eval_utils_calvin import BatchedRolloutEngine, RolloutEngine
 
 
 def quaternion_to_euler(q):
@@ -88,3 +88,70 @@ class ModelWrapper(RolloutEngine):
             action = act.to(torch.float16).cpu().numpy()
         self.gripper_state = np.array([float(action[-1])])                    # :178
         return action
+
+
+class BatchedModelWrapper(BatchedRolloutEngine):
+    """LIBERO rollout wrapper for `num_envs` environments: `ModelWrapper.step` per env, batched (see BatchedRolloutEngine).
+    Per env: the agent-view flip, the 7- or 8-dim (`gripper_width`) state, the gripper command fed back from the previous
+    action and the temporal-ensembling buffer."""
+
+    def __init__(self, model, num_envs, cast_dtype=torch.bfloat16, history_len=7, use_ensembling=False, ensembling_temp=0.01,
+                 libero_eval_max_steps=600, action_pred_steps=3, gripper_width=False, device="cuda", use_cuda_graph=True,
+                 incremental=True):
+        super().__init__(model, num_envs, cast_dtype, history_len, action_pred_steps, device, use_cuda_graph, incremental,
+                         state_dim=8 if gripper_width else 7)
+        self.use_ensembling = use_ensembling
+        self.ensembling_temp = ensembling_temp
+        self.libero_eval_max_steps = libero_eval_max_steps
+        self.gripper_width = gripper_width
+        self.gripper_state = [np.array([-1.0]) for _ in range(num_envs)]
+        self.all_time_actions = [self._ensemble_buffer() if use_ensembling else None for _ in range(num_envs)]
+
+    def _ensemble_buffer(self):
+        return torch.zeros([self.libero_eval_max_steps, self.libero_eval_max_steps + self.action_pred_steps, 7],
+                           device=self.device)
+
+    def reset(self, env):                                                   # :80-92
+        self.reset_window(env)
+        self.gripper_state[env] = np.array([-1.0])
+        if self.use_ensembling:
+            self.all_time_actions[env] = self._ensemble_buffer()
+
+    def build_state(self, env, eef_pos, eef_quat, gripper_qpos=None):
+        pos, ori = np.asarray(eef_pos, dtype=np.float64), quaternion_to_euler(eef_quat)
+        if not self.gripper_width:
+            return np.concatenate([pos, ori, self.gripper_state[env]])
+        return np.concatenate([pos, ori, np.asarray(gripper_qpos, dtype=np.float64)])
+
+    @torch.no_grad()
+    def step(self, envs, image_agentview, image_eye_in_hand, eef_pos, eef_quat, gripper_qpos, text_tokens, timesteps,
+             sample_noise=None):
+        """One env step for each env in `envs` -> actions [n, 7] numpy (see ModelWrapper.step; per-env arguments stacked or
+        listed in the order of `envs`, gripper_qpos may be None without gripper_width)."""
+        n = len(envs)
+        qpos = gripper_qpos if gripper_qpos is not None else [None] * n
+        state = torch.from_numpy(np.stack([self.build_state(e, eef_pos[i], eef_quat[i], qpos[i]) for i, e in enumerate(envs)]))
+        arm, gripper, _ = self.infer_batch(envs, image_agentview, image_eye_in_hand, state, text_tokens, sample_noise,
+                                           flip_static=True)
+        actions = []
+        for i, e in enumerate(envs):
+            t = int(timesteps[i])
+            if self.use_ensembling:
+                buf = self.all_time_actions[e]
+                action = torch.cat((arm[i], gripper[i]), dim=-1).unsqueeze(0)        # (1, action_pred_steps, 7)   :165
+                buf[t:t + 1, t:t + self.action_pred_steps] = action.to(buf.dtype)
+                cur = buf[:, t]
+                cur = cur[torch.all(cur != 0, dim=1)]
+                w = np.exp(-self.ensembling_temp * np.arange(len(cur)))
+                w = torch.from_numpy(w / w.sum()).to(self.device).unsqueeze(1)
+                act = (cur * w).sum(dim=0, keepdim=True)
+                act = torch.cat((act[:, :6], (act[:, 6:] > 0.5).to(act.dtype)), dim=-1)
+                act[:, -1] = (act[:, -1] - 0.5) * 2
+                a = act.detach().cpu().numpy()[-1]
+            else:
+                act = torch.cat((arm[i, 0].float(), (gripper[i, 0] > 0.5).float()), dim=-1)
+                act[-1] = (act[-1] - 0.5) * 2
+                a = act.to(torch.float16).cpu().numpy()
+            self.gripper_state[e] = np.array([float(a[-1])])                     # :178
+            actions.append(a)
+        return np.stack(actions)

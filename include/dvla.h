@@ -158,6 +158,14 @@ typedef struct {
                                  (dreamvla_model.py:803-806 with an all-zero position embedding).  Short-sequence kernels only
                                  (Lq <= 32, Lk <= 64, no mask, no dropout); DVLA_ERR_UNSUPPORTED otherwise. */
   int64_t head_dim;           /* 0 or 64, or 96 on the short-sequence kernels (see above) */
+  /* Per-sequence masks (appended after version 100 shipped; NULL keeps the meaning above): `mask` and `tile_flags` are the
+   * first of a stack of bit matrices / tile-flag arrays of one shape, and batch b attends under
+   * mask + mask_index[b] * mask_stride with tile_flags + mask_index[b] * flags_stride.  mask_index is DEVICE int32 [B]; its
+   * values must select matrices inside the caller's stack (not checked: the kernels read them).  Both mma.sync and wgmma
+   * forward kernels honour it; a mask_index without a mask is DVLA_ERR_INVALID, as are negative strides. */
+  const int32_t* mask_index;
+  int64_t mask_stride;        /* uint32 words between consecutive bit matrices */
+  int64_t flags_stride;       /* bytes between consecutive tile-flag arrays */
 } dvla_attn_fwd_args;
 int dvla_attn_fwd(const dvla_attn_fwd_args* args, void* stream);
 
@@ -280,8 +288,10 @@ int dvla_grad_clip_scale(void* g_bf16, int64_t n, const float* sumsq, float max_
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Fused action sampler: the DDIM loop of the DiT action head with classifier-free guidance as ONE persistent cooperative
- * kernel (replaces dreamvla_model.py:935-987 -> gaussian_diffusion.py:609-689 -> models.py:253-268 for small batches:
- * rows = 2 * batch * 2T <= 24).  Every pointer is device memory, weights are bf16 nn.Linear layouts [out, in].
+ * kernel (replaces dreamvla_model.py:935-987 -> gaussian_diffusion.py:609-689 -> models.py:253-268 for small batches).
+ * rows = 2 * batch * 2T with 2T = 6: batch 1 (12 rows, FMA GEMMs) or 2 <= batch <= 8 (up to 96 rows, tensor-core GEMMs; hidden,
+ * token and freq multiples of 32, mlp a multiple of hidden); a batch above 8 returns DVLA_ERR_UNSUPPORTED before any launch.
+ * Every pointer is device memory, weights are bf16 nn.Linear layouts [out, in].
  * head_dim = hidden / heads must be 64 (DiT-B, DiT-L) or 96 (DiT-S); DVLA_ERR_UNSUPPORTED otherwise.
  * Schedule tables are HOST arrays of n_steps entries (respaced DDIM: timestep_map[i] is the original timestep of step i).
  * n_steps <= 12 (the prologue embeds every step's timestep as one row of a 12-row GEMM); DVLA_ERR_UNSUPPORTED otherwise.
