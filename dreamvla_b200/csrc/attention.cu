@@ -733,12 +733,23 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const AttnParams p) {
 //                register A operand, Q / dO read MN-major)
 //   DKV = false: CTA = query tiles 2x, 2x+1; group g owns query tile 2x+g (Q, dO) and streams key tiles (K, V):
 //                S = Q K^T, dP = dO V^T, dQ += dS K
-// Warp 8 is the TMA producer (3-stage ring of streamed tile pairs); a streamed tile is loaded when either group sees it.
+// Warpgroup 2 is the producer (3-stage ring of streamed tile pairs); a streamed tile is loaded when either group sees it.
+// Its thread 0 issues the TMA loads.  In the dK/dV kernel all 128 of its threads also fill the stage's row statistics
+// (below) before they arrive on the stage's full barrier, so the consumers read each query's lse, delta, mask word and
+// dropout keep bits with one shared load per two queries instead of per element.  setmaxnreg hands the producer's
+// registers to the consumers, which hold dK, dV, S^T and dP^T (128 x 56 + 256 x 224 registers <= 64 K; at 40 the
+// producer's Philox draws spill).
 struct WgmmaBwdMaps { CUtensorMap f0, f1, s0, s1; int f0_hi, f1_hi, s0_hi, s1_hi; };
+constexpr int WB_THREADS = 384;
+// Row statistics of one stage's query tile, in 32-bit words: lse * log2(e) and delta of its 64 queries (+inf and 0 past
+// Lq), then per consumer group g and mask word ww of its key tile the words [g][ww][query] of the bit mask and of the
+// dropout keep bits.  Keep word ww of a query packs its 8-key Philox blocks 4 ww .. 4 ww + 3, the forward's blocks, so
+// bit (key & 31) of word key / 32 is the key's keep bit, as in the mask.
+constexpr int WB_STAT_LSE = 0, WB_STAT_DELTA = 64, WB_STAT_MASK = 128, WB_STAT_KEEP = 384, WB_STAT_WORDS = 640;
 
 template <bool DKV>
-// One CTA per SM: dK and dV accumulators next to S and dP need ~160 registers (two CTAs of 9 warps cap a thread at 96).
-__global__ void __launch_bounds__(WF_THREADS, 1) attn_bwd_wgmma_kernel(const __grid_constant__ WgmmaBwdMaps tm, const AttnParams p) {
+// One CTA per SM: dK and dV accumulators next to S and dP need ~160 registers.
+__global__ void __launch_bounds__(WB_THREADS, 1) attn_bwd_wgmma_kernel(const __grid_constant__ WgmmaBwdMaps tm, const AttnParams p) {
   extern __shared__ uint8_t wb_smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(wb_smem_raw) + 1023) & ~uintptr_t(1023));
   const uint32_t sF = smem_u32(smem);                       // [group][f0 8 KB | f1 8 KB]
@@ -747,6 +758,7 @@ __global__ void __launch_bounds__(WF_THREADS, 1) attn_bwd_wgmma_kernel(const __g
   uint64_t* f_full = bars;
   uint64_t* full = bars + 1;
   uint64_t* empty = full + WF_STAGES;
+  uint32_t* stats = reinterpret_cast<uint32_t*>(smem + 4 * 8192 + WF_STAGES * 2 * 8192 + 128);   // [stage][WB_STAT_WORDS]
   const int h = blockIdx.x, b = blockIdx.y;
   const int nf = DKV ? p.nkt : p.nqt;                       // tiles on the fixed side
   const int ns = DKV ? p.nqt : p.nkt;                       // tiles on the streamed side
@@ -769,35 +781,72 @@ __global__ void __launch_bounds__(WF_THREADS, 1) attn_bwd_wgmma_kernel(const __g
 
   if (threadIdx.x == 0) {
     mbar_init(f_full, 1);
-    for (int st = 0; st < WF_STAGES; ++st) { mbar_init(&full[st], 1); mbar_init(&empty[st], 8); }
+    // dK/dV: the TMA thread's expect_tx arrival and one arrival per producer thread once its statistics are written
+    for (int st = 0; st < WF_STAGES; ++st) { mbar_init(&full[st], DKV ? 1 + 128 : 1); mbar_init(&empty[st], 8); }
     fence_barrier_init();
   }
   __syncthreads();
+  const long long bh = static_cast<long long>(b) * p.H + h;
 
-  if (warp == 8) {
-    if (lane == 0) {
+  if (warp >= 8) {
+    setmaxnreg_dec<56>();
+    const int pt = threadIdx.x - 256;
+    if (!DKV && pt != 0) return;
+    if (pt == 0) {
       tma_prefetch_desc(&tm.f0); tma_prefetch_desc(&tm.f1); tma_prefetch_desc(&tm.s0); tma_prefetch_desc(&tm.s1);
       mbar_expect_tx(f_full, 4 * 8192);
       for (int g = 0; g < 2; ++g) {                         // a tile past the sequence end is zero-filled
         tma_rows(sF + g * 16384, &tm.f0, f_full, tm.f0_hi, (ft_base + g) * 64, h, b);
         tma_rows(sF + g * 16384 + 8192, &tm.f1, f_full, tm.f1_hi, (ft_base + g) * 64, h, b);
       }
-      int st = 0; uint32_t ph = 0;
-      for (int t = next_tile(0); t < ns; t = next_tile(t + 1)) {
-        mbar_wait<false>(&empty[st], ph ^ 1);
+    }
+    const uint64_t seed = p.drop_seed + (p.drop_seed_ptr ? __ldg(p.drop_seed_ptr) : 0ull);
+    const int nblk = (p.Lk + 7) >> 3;
+    int st = 0; uint32_t ph = 0;
+    for (int t = next_tile(0); t < ns; t = next_tile(t + 1)) {
+      mbar_wait<false>(&empty[st], ph ^ 1);
+      if (pt == 0) {
         mbar_expect_tx(&full[st], 2 * 8192);
         tma_rows(sS + st * 16384, &tm.s0, &full[st], tm.s0_hi, t * 64, h, b);
         tma_rows(sS + st * 16384 + 8192, &tm.s1, &full[st], tm.s1_hi, t * 64, h, b);
-        if (++st == WF_STAGES) { st = 0; ph ^= 1; }
       }
+      if (DKV) {
+        // thread pt: lse (pt < 64) or delta (pt >= 64) of query pt % 64; mask and keep words of query pt % 64 for
+        // consumer group pt / 64, written only where that group reads them (flag 1 / flag != 0 with dropout)
+        uint32_t* sw = stats + st * WB_STAT_WORDS;
+        const int qc = pt & 63, gg = pt >> 6;
+        const int qi = t * 64 + qc;
+        const bool qin = qi < p.Lq;
+        if (pt < 64) reinterpret_cast<float*>(sw)[WB_STAT_LSE + qc] = qin ? p.lse[bh * p.Lq + qi] * LOG2E : INFINITY;
+        else         reinterpret_cast<float*>(sw)[WB_STAT_DELTA + qc] = qin ? p.delta[bh * p.Lq + qi] : 0.f;
+        const int flag = flag_of(t, gg);
+        const int kb0 = (ft_base + gg) * 8;                 // first 8-key block of the group's key tile
+#pragma unroll
+        for (int ww = 0; ww < 2; ++ww) {
+          const int slot = (gg * 2 + ww) * 64 + qc;
+          if (flag == 1) {
+            const int wi = (kb0 >> 2) + ww;
+            sw[WB_STAT_MASK + slot] = (qin && wi < p.mask_words) ? __ldg(p.mask + static_cast<long long>(qi) * p.mask_words + wi) : 0u;
+          }
+          if (flag != 0 && p.drop_scale != 0.f) {
+            uint32_t kw = 0;
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+              kw |= dropout_keep8(seed, (bh * p.Lq + qi) * nblk + kb0 + ww * 4 + j, p.drop_thresh) << (8 * j);
+            sw[WB_STAT_KEEP + slot] = kw;
+          }
+        }
+        mbar_arrive(&full[st]);
+      }
+      if (++st == WF_STAGES) { st = 0; ph ^= 1; }
     }
     return;
   }
 
+  setmaxnreg_inc<224>();
   const int g = warp >> 2, wq = warp & 3;
   const int c = lane & 3, gr = lane >> 2;
   const int f0 = (ft_base + g) * 64;                        // first key (DKV) / query (dQ) row of this group
-  const long long bh = static_cast<long long>(b) * p.H + h;
   const float sc = p.scale * LOG2E;
   const uint32_t fa0 = sF + g * 16384, fa1 = fa0 + 8192;   // DKV: K, V of the key tile; dQ: Q, dO of the query tile
   float acc0[8][4], acc1[8][4];                             // DKV: dK, dV; dQ: dQ (acc1 unused)
@@ -829,38 +878,36 @@ __global__ void __launch_bounds__(WF_THREADS, 1) attn_bwd_wgmma_kernel(const __g
       wgmma_fence_operand32(sd);
       wgmma_fence_operand32(dpd);
       if (DKV) {
-        // ---- as attn_bwd_dkv_kernel: rows = keys (f0 + ...), cols = queries (s0r + ...).  Not shared with it: a
-        // helper taking the query's lse / delta / mask word through lambdas made this kernel 2.5-4% slower on an H100 ----
-        const int k0 = f0, q0 = s0r;
-        uint32_t keep[8];
-        if (p.drop_scale != 0.f) dropout_bits(p, bh, k0 + wq * 16, q0, true, keep);
-        const int ww = wq >> 1;                               // mask word of this warp's 16 key rows
+        // ---- as attn_bwd_dkv_kernel: rows = keys (f0 + ...), cols = queries (s0r + ...), with the query's lse, delta,
+        // mask word and keep bits from the stage's statistics (the producer wrote them before the full barrier) ----
+        const int k0 = f0;
+        const uint32_t* sw = stats + st * WB_STAT_WORDS;
+        const int slot = (g * 2 + (wq >> 1)) * 64;            // mask / keep word of this warp's 16 key rows
         float pt[8][4];
 #pragma unroll
         for (int tt = 0; tt < 8; ++tt) {
+          const int qc = tt * 8 + 2 * c;                      // this thread's queries qc, qc + 1 of the tile
+          const float2 lse_q = *reinterpret_cast<const float2*>(sw + WB_STAT_LSE + qc);
+          const float2 dlt_q = *reinterpret_cast<const float2*>(sw + WB_STAT_DELTA + qc);
+          uint2 mw = make_uint2(0u, 0u), kw = make_uint2(0u, 0u);
+          if (flag == 1) mw = *reinterpret_cast<const uint2*>(sw + WB_STAT_MASK + slot + qc);
+          if (p.drop_scale != 0.f) kw = *reinterpret_cast<const uint2*>(sw + WB_STAT_KEEP + slot + qc);
 #pragma unroll
           for (int e = 0; e < 4; ++e) {
             const int kr = wq * 16 + gr + (e >> 1) * 8;
-            const int qi = q0 + tt * 8 + 2 * c + (e & 1);
-            const bool qin = qi < p.Lq;
-            const float lse_q = qin ? p.lse[bh * p.Lq + qi] * LOG2E : INFINITY;
-            const float dlt_q = qin ? p.delta[bh * p.Lq + qi] : 0.f;
+            const float lse_e = (e & 1) ? lse_q.y : lse_q.x, dlt_e = (e & 1) ? dlt_q.y : dlt_q.x;
             bool vis = (k0 + kr < p.Lk);
-            if (flag == 1) {
-              const int wi = (k0 >> 5) + ww;
-              const uint32_t mw = (qin && wi < p.mask_words) ? __ldg(p.mask + static_cast<long long>(qi) * p.mask_words + wi) : 0u;
-              vis = vis && ((mw >> (kr & 31)) & 1u);
-            }
-            const float pv = vis ? exp2f(s[tt][e] * sc - lse_q) : 0.f;
+            if (flag == 1) vis = vis && ((((e & 1) ? mw.y : mw.x) >> (kr & 31)) & 1u);
+            const float pv = vis ? exp2f(s[tt][e] * sc - lse_e) : 0.f;
             float dpv = dp[tt][e];
             float pdrop = pv;
             if (p.drop_scale != 0.f) {
-              const bool kp = (keep[tt] >> e) & 1u;
+              const bool kp = ((((e & 1) ? kw.y : kw.x) >> (kr & 31)) & 1u);
               pdrop = kp ? pv * p.drop_scale : 0.f;
               dpv = kp ? dpv * p.drop_scale : 0.f;
             }
             pt[tt][e] = pdrop;
-            s[tt][e] = pv * (dpv - dlt_q);
+            s[tt][e] = pv * (dpv - dlt_e);
           }
         }
         uint32_t pa[4][4], da[4][4];
@@ -903,7 +950,7 @@ __global__ void __launch_bounds__(WF_THREADS, 1) attn_bwd_wgmma_kernel(const __g
     store_frag_bf16(p.dq + b * p.dq_sb + h * p.dq_sh, p.dq_ss, f0 + wq * 16, p.Lq, acc0, p.scale);
   }
 }
-constexpr int WB_SMEM = 1024 + 4 * 8192 + WF_STAGES * 2 * 8192 + 128;
+constexpr int WB_SMEM = 1024 + 4 * 8192 + WF_STAGES * 2 * 8192 + 128 + WF_STAGES * WB_STAT_WORDS * 4;
 
 // ===================================================== mask tiles =================================================
 __global__ void attn_mask_tiles_kernel(const uint32_t* __restrict__ mask, int mask_words, int Lq, int Lk, int nkt,
@@ -1040,7 +1087,7 @@ static int attn_bwd_wgmma_launch(const WgmmaBwdMaps& tm, const AttnParams& p, cu
   static cudaError_t attr_err = cudaSuccess;
   if (!set_smem_attr_once(once, attr_err, attn_bwd_wgmma_kernel<DKV>, WB_SMEM)) { set_error("attn_bwd_wgmma smem attribute: %s", cudaGetErrorString(attr_err)); return DVLA_ERR_CUDA; }
   const int nf = DKV ? p.nkt : p.nqt;
-  attn_bwd_wgmma_kernel<DKV><<<dim3(p.H, p.B, (nf + 1) / 2), WF_THREADS, WB_SMEM, s>>>(tm, p);
+  attn_bwd_wgmma_kernel<DKV><<<dim3(p.H, p.B, (nf + 1) / 2), WB_THREADS, WB_SMEM, s>>>(tm, p);
   DVLA_CHECK_LAUNCH(DKV ? "attn_bwd_dkv_wgmma" : "attn_bwd_dq_wgmma");
   return DVLA_OK;
 }
