@@ -6,7 +6,7 @@
 // Why: at batch 1 the sampler is 10 x (12 DiT blocks + embedders + final layer + DDIM algebra) ~ 1100 kernel launches on
 // 12 token rows (2 guidance branches x 6 tokens) -- every launch is latency, none is work: the whole DiT-B is 170 MB of bf16
 // weights, i.e. ~30 us per pass at HBM speed.  The same kernel runs DiT-S (head_dim 96) and DiT-L (depth 24, hidden 1024).  Here one CTA per SM stays resident for the entire sample; every linear layer
-// is a "skinny" GEMM (M <= 24 rows) in which a warp owns one output column, streams that column's weight row from HBM/L2
+// is a "skinny" GEMM (M = 12 rows) in which a warp owns one output column, streams that column's weight row from HBM/L2
 // with 16-byte loads and keeps the activations (bf16) in shared memory; the phases of a block (LN+QKV | attention+proj+res |
 // LN+fc1+GELU | fc2+res) are separated by grid barriers (cooperative launch) instead of kernel boundaries.  Timestep and
 // condition embeddings are hoisted out of the loop (they do not depend on x); x itself (T x 7 numbers per sample) lives in
@@ -31,9 +31,7 @@ namespace {
 
 constexpr int DS_THREADS = 512;      // 16 warps per SM: the skinny GEMMs hide weight-load latency with warps in flight
 constexpr int DS_WARPS = DS_THREADS / 32;
-constexpr int DS_MAXM = 12;          // rows of one sequence: 2 guidance branches x 2T tokens (the batch-1 rollout case)
-constexpr int DS_MAXB = 8;           // sequences of the multi-sequence bucket
-constexpr int DS_ROWS_TC = 96;       // its rows: 2 x DS_MAXB x 6 tokens, on the tensor-core GEMM (skinny_gemm_tc)
+constexpr int DS_MAXM = 12;          // rows of one sequence: 2 guidance branches x 2T tokens (batch 1; larger batches use the module path)
 constexpr int DS_MAX_DEPTH = 28;
 constexpr int DS_MAX_STEPS = 16;
 
@@ -54,7 +52,6 @@ struct DitSamplerParams {
   // flow matching only (behind the DDIM fields, whose parameter offsets -- and so the DDIM code -- stay as they were)
   float tval[DS_MAX_STEPS];  // DiT timestep input of step i, in execution order
   float fm_delta;            // Euler step 1 / n_steps
-  long long xs_elems;        // multi-sequence bucket: bf16 elements of the staging area in front of xcur
 };
 
 __device__ __forceinline__ float gelu_tanh_f(float x) {
@@ -185,105 +182,6 @@ __device__ __noinline__ void skinny_gemm(const bf16* __restrict__ Xs, int M, int
   }
 }
 
-__device__ __forceinline__ void ds_mma16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
-// The same product and epilogues for the multi-sequence bucket (M <= 96 rows): at 96 rows the FMA body above needs 192
-// accumulators per lane and no longer hides behind the weight stream, so the rows go through mma.sync.m16n8k16 (bf16 in, fp32
-// accumulate).  A warp owns 16 output columns (two n8 tiles) over all six m16 tiles and streams the two weight row groups
-// from HBM / L2 with 16-byte loads, four 32-wide k chunks in flight.  Inside a chunk, lane quad position c takes the 8
-// consecutive k's [8c, 8c + 8) for both operands (a permutation of the chunk's k order, the same for A and B, so the sum is
-// unchanged): one 16-byte load of W and one of each staged row feed two k16 steps.  W rows have stride ldw (fc2 is run on
-// K chunks of its input); K % 32 == 0, N % 16 == 0.  EPI_ACC with few column groups splits K over idle warps with fp32
-// atomics, as skinny_gemm does.  One out-of-line copy, like skinny_gemm.
-__device__ __noinline__ void skinny_gemm_tc(const bf16* __restrict__ Xs, int M, int K, const bf16* __restrict__ W, int ldw,
-                                            const bf16* __restrict__ bias, int N, float* __restrict__ out, int ldo, int mode) {
-  constexpr int MT = DS_ROWS_TC / 16;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, c = lane & 3;
-  const int gw = blockIdx.x * DS_WARPS + warp, nw = gridDim.x * DS_WARPS;
-  const int chunks = K >> 5, groups = N >> 4;
-  int ksplit = 1;
-  if (mode == EPI_ACC && nw >= 2 * groups) {
-    ksplit = nw / groups;
-    if (ksplit > chunks / 4) ksplit = chunks / 4;
-    if (ksplit < 1) ksplit = 1;
-  }
-  for (int unit = gw; unit < groups * ksplit; unit += nw) {
-    const int grp = unit % groups, ks = unit / groups;
-    const int cb = (chunks * ks) / ksplit, ce = (chunks * (ks + 1)) / ksplit;
-    const int n0 = grp * 16;
-    float acc[MT][2][4];
-#pragma unroll
-    for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-      for (int t = 0; t < 2; ++t)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) acc[mt][t][e] = 0.f;
-    const bf16* w0 = W + static_cast<long long>(n0 + g) * ldw + c * 8;
-    const bf16* w1 = w0 + 8LL * ldw;
-    for (int k0 = cb; k0 < ce; k0 += 4) {
-      uint4 b0[4], b1[4];
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        const bool ok = k0 + u < ce;
-        b0[u] = ok ? __ldg(reinterpret_cast<const uint4*>(w0 + (k0 + u) * 32)) : make_uint4(0, 0, 0, 0);
-        b1[u] = ok ? __ldg(reinterpret_cast<const uint4*>(w1 + (k0 + u) * 32)) : make_uint4(0, 0, 0, 0);
-      }
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        if (k0 + u >= ce) break;
-        const int kk = (k0 + u) * 32 + c * 8;
-#pragma unroll
-        for (int mt = 0; mt < MT; ++mt) {
-          if (mt * 16 >= M) break;
-          const int r0 = min(mt * 16 + g, M - 1), r1 = min(mt * 16 + 8 + g, M - 1);   // rows past M: any staged row
-          const uint4 x = *reinterpret_cast<const uint4*>(Xs + r0 * K + kk);
-          const uint4 y = *reinterpret_cast<const uint4*>(Xs + r1 * K + kk);
-          const uint32_t a0[4] = {x.x, y.x, x.y, y.y}, a1[4] = {x.z, y.z, x.w, y.w};
-          ds_mma16816(acc[mt][0], a0, b0[u].x, b0[u].y);
-          ds_mma16816(acc[mt][1], a0, b1[u].x, b1[u].y);
-          ds_mma16816(acc[mt][0], a1, b0[u].z, b0[u].w);
-          ds_mma16816(acc[mt][1], a1, b1[u].z, b1[u].w);
-        }
-      }
-    }
-    // C fragment: acc[mt][t][2h + e] is row mt*16 + g + 8h, column n0 + 8t + 2c + e
-#pragma unroll
-    for (int mt = 0; mt < MT; ++mt) {
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        const int row = mt * 16 + g + 8 * hh;
-        if (row >= M) continue;
-#pragma unroll
-        for (int t = 0; t < 2; ++t)
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int n = n0 + 8 * t + 2 * c + e;
-            float v = acc[mt][t][2 * hh + e] + ((bias && ks == 0) ? __bfloat162float(bias[n]) : 0.f);
-            float* dst = out + static_cast<long long>(row) * ldo + n;
-            if (ksplit > 1) { atomicAdd(dst, v); continue; }
-            if (mode == EPI_SILU) v = v / (1.0f + __expf(-v));
-            else if (mode == EPI_GELU) v = gelu_tanh_f(v);
-            else if (mode == EPI_ACC) v += __ldcg(dst);
-            __stcg(dst, v);
-          }
-      }
-    }
-  }
-}
-
-// The GEMM of row bucket MROWS: the FMA body up to DS_MAXM rows, the tensor-core one above.
-template <int MROWS>
-__device__ __forceinline__ void ds_gemm(const bf16* Xs, int M, int K, const bf16* W, const bf16* bias, int N, float* out, int ldo,
-                                        int mode) {
-  if constexpr (MROWS > DS_MAXM) skinny_gemm_tc(Xs, M, K, W, K, bias, N, out, ldo, mode);
-  else skinny_gemm<MROWS>(Xs, M, K, W, bias, N, out, ldo, mode);
-}
-
 // Xs[m][:] = bf16(LayerNorm(h[m][:])) without affine, eps 1e-6 (timm Block with elementwise_affine=False).  Warp per row; the row
 // is fetched ONCE with independent 16-byte ld.global.cg loads (up to 8 per lane, H <= 1024) and normalised from registers:
 // three dependent scalar passes over L2 cost ~10 us per phase.
@@ -362,8 +260,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dit_ddim_sample_kernel(const __
   const int nseq = 2 * bs;             // guidance: sequences [0, bs) conditional, [bs, 2bs) unconditional (models.py:253-257)
   const int M = nseq * L;
   bf16* Xs = reinterpret_cast<bf16*>(ds_smem);                                // staged GEMM input, up to [M][mlp]
-  const size_t xs_elems = MROWS > DS_MAXM ? static_cast<size_t>(p.xs_elems) : static_cast<size_t>(M) * p.mlp;
-  float* xcur = reinterpret_cast<float*>(ds_smem + xs_elems * 2);                // [bs][T][C] current sample
+  float* xcur = reinterpret_cast<float*>(ds_smem + static_cast<size_t>(M) * p.mlp * 2);     // [bs][T][C] current sample
   float* eps_s = xcur + bs * T * C;                                           // [nseq][T][C] final-layer outputs
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int gtid = blockIdx.x * DS_THREADS + tid, gthreads = gridDim.x * DS_THREADS;
@@ -377,7 +274,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dit_ddim_sample_kernel(const __
     Xs[i] = __float2bfloat16(k < half ? cosf(a) : sinf(a));
   }
   __syncthreads();
-  ds_gemm<MROWS>(Xs, p.n_steps, p.freq, p.t0_w, p.t0_b, H, p.t1, H, EPI_SILU);
+  skinny_gemm<MROWS>(Xs, p.n_steps, p.freq, p.t0_w, p.t0_b, H, p.t1, H, EPI_SILU);
   __syncthreads();
   {
     const int rows = bs * T + 1;
@@ -386,14 +283,14 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dit_ddim_sample_kernel(const __
       Xs[i] = r < bs * T ? p.z[static_cast<long long>(r) * p.token + k] : p.uncond[k];
     }
     __syncthreads();
-    ds_gemm<MROWS>(Xs, rows, p.token, p.z_w, p.z_b, H, p.ze, H, EPI_STORE);
+    skinny_gemm<MROWS>(Xs, rows, p.token, p.z_w, p.z_b, H, p.ze, H, EPI_STORE);
   }
   for (int i = tid; i < bs * T * C; i += DS_THREADS) xcur[i] = FM ? p.noise[i] : __bfloat162float(__float2bfloat16(p.noise[i]));
   grid.sync();
   // ---- prologue B: te = W2 t1 + b2
   stage_rows(Xs, p.t1, p.n_steps * H);
   __syncthreads();
-  ds_gemm<MROWS>(Xs, p.n_steps, H, p.t2_w, p.t2_b, H, p.te, H, EPI_STORE);
+  skinny_gemm<MROWS>(Xs, p.n_steps, H, p.t2_w, p.t2_b, H, p.te, H, EPI_STORE);
   grid.sync();
 
   for (int step = FM ? 0 : p.n_steps - 1, it = 0; FM ? step < p.n_steps : step >= 0; step += FM ? 1 : -1, ++it) {
@@ -421,7 +318,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dit_ddim_sample_kernel(const __
       // ---- P1: qkv = LN(h) Wqkv^T + b
       stage_layernorm(Xs, h, M, H);
       __syncthreads();
-      ds_gemm<MROWS>(Xs, M, H, w.qkv_w, w.qkv_b, 3 * H, p.qkv, 3 * H, EPI_STORE);
+      skinny_gemm<MROWS>(Xs, M, H, w.qkv_w, w.qkv_b, 3 * H, p.qkv, 3 * H, EPI_STORE);
       grid.sync();
       // ---- P2: attention (every CTA computes all (sequence, head) pairs: 6x6 scores each) -> O in shared; h += O Wproj^T + b
       {
@@ -473,31 +370,18 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dit_ddim_sample_kernel(const __
           }
         }
         __syncthreads();
-        ds_gemm<MROWS>(Os, M, H, w.proj_w, w.proj_b, H, h, H, EPI_ACC);
+        skinny_gemm<MROWS>(Os, M, H, w.proj_w, w.proj_b, H, h, H, EPI_ACC);
       }
       grid.sync();
       // ---- P3: u = gelu_tanh(LN(h) Wfc1^T + b)
       stage_layernorm(Xs, h, M, H);
       __syncthreads();
-      ds_gemm<MROWS>(Xs, M, H, w.fc1_w, w.fc1_b, p.mlp, p.u, p.mlp, EPI_GELU);
+      skinny_gemm<MROWS>(Xs, M, H, w.fc1_w, w.fc1_b, p.mlp, p.u, p.mlp, EPI_GELU);
       grid.sync();
-      // ---- P4: h += u Wfc2^T + b  (multi-sequence bucket: [M][mlp] does not fit shared memory, so K chunks of H columns)
-      if constexpr (MROWS > DS_MAXM) {
-        for (int k0 = 0; k0 < p.mlp; k0 += H) {
-          for (int i = tid; i < M * (H >> 2); i += DS_THREADS) {
-            const int r = i / (H >> 2), c4 = i - r * (H >> 2);
-            const float4 v = __ldcg(reinterpret_cast<const float4*>(p.u + static_cast<long long>(r) * p.mlp + k0) + c4);
-            reinterpret_cast<uint2*>(Xs + r * H)[c4] = make_uint2(pack_bf16x2(v.x, v.y), pack_bf16x2(v.z, v.w));
-          }
-          __syncthreads();
-          skinny_gemm_tc(Xs, M, H, w.fc2_w + k0, p.mlp, k0 == 0 ? w.fc2_b : nullptr, H, h, H, EPI_ACC);
-          __syncthreads();
-        }
-      } else {
-        stage_rows(Xs, p.u, M * p.mlp);
-        __syncthreads();
-        skinny_gemm<MROWS>(Xs, M, p.mlp, w.fc2_w, w.fc2_b, H, h, H, EPI_ACC);
-      }
+      // ---- P4: h += u Wfc2^T + b
+      stage_rows(Xs, p.u, M * p.mlp);
+      __syncthreads();
+      skinny_gemm<MROWS>(Xs, M, p.mlp, w.fc2_w, w.fc2_b, H, h, H, EPI_ACC);
       grid.sync();
     }
     // ---- final layer on the action rows + guidance + DDIM / Euler update: redundantly in every CTA (x stays in shared memory).
@@ -539,17 +423,16 @@ __global__ void __launch_bounds__(DS_THREADS, 1) dit_ddim_sample_kernel(const __
 }
 
 // The instantiation the host launches; the shared-memory opt-in is made once per instantiation.
-template <int MROWS, int HD, int INTEG>
+template <int HD, int INTEG>
 void* sampler_kernel(cudaError_t* attr_err) {
   static const cudaError_t e =
-      cudaFuncSetAttribute(dit_ddim_sample_kernel<MROWS, 6, HD, INTEG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+      cudaFuncSetAttribute(dit_ddim_sample_kernel<DS_MAXM, 6, HD, INTEG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
   *attr_err = e;
-  return reinterpret_cast<void*>(dit_ddim_sample_kernel<MROWS, 6, HD, INTEG>);
+  return reinterpret_cast<void*>(dit_ddim_sample_kernel<DS_MAXM, 6, HD, INTEG>);
 }
-template <int MROWS>
 void* sampler_kernel_for(int64_t head_dim, bool fm, cudaError_t* attr_err) {
-  return head_dim == 96 ? (fm ? sampler_kernel<MROWS, 96, DS_FM>(attr_err) : sampler_kernel<MROWS, 96, DS_DDIM>(attr_err))
-                        : (fm ? sampler_kernel<MROWS, 64, DS_FM>(attr_err) : sampler_kernel<MROWS, 64, DS_DDIM>(attr_err));
+  return head_dim == 96 ? (fm ? sampler_kernel<96, DS_FM>(attr_err) : sampler_kernel<96, DS_DDIM>(attr_err))
+                        : (fm ? sampler_kernel<64, DS_FM>(attr_err) : sampler_kernel<64, DS_DDIM>(attr_err));
 }
 
 }  // namespace
@@ -570,20 +453,17 @@ extern "C" int dvla_dit_ddim_sample(const dvla_dit_sampler_args* a, void* stream
   if (a->n_steps > DS_MAXM) {
     set_error("dit_ddim_sample: n_steps %lld above the %d prologue rows", (long long)a->n_steps, DS_MAXM); return DVLA_ERR_UNSUPPORTED;
   }
-  if (a->batch < 1 || a->batch > DS_MAXB) {
-    set_error("dit_ddim_sample: batch %lld outside 1 .. %d sequences", (long long)a->batch, DS_MAXB); return DVLA_ERR_UNSUPPORTED;
+  if (a->batch != 1) {
+    set_error("dit_ddim_sample: batch %lld unsupported: the fused sampler samples one sequence (batch 1)", (long long)a->batch);
+    return DVLA_ERR_UNSUPPORTED;
   }
   const int H = (int)a->hidden, T = (int)a->T, C = (int)a->channels, bs = (int)a->batch;
   const int M = 2 * bs * 2 * T;
-  const bool multi = bs > 1;                        // the multi-sequence bucket: tensor-core GEMMs, fc2 on K chunks of H
-  const int maxm = multi ? DS_ROWS_TC : DS_MAXM;
   const int64_t head_dim = a->heads > 0 && a->hidden % a->heads == 0 ? a->hidden / a->heads : 0;
-  if (a->depth <= 0 || a->depth > DS_MAX_DEPTH || a->n_steps <= 0 || a->n_steps > DS_MAX_STEPS || M > maxm || 2 * T > 8 ||
-      (head_dim != 64 && head_dim != 96) || H % 8 || a->token % 8 || a->mlp % 8 || a->freq % 8 || bs * T + 1 > maxm ||
-      (multi && (H % 32 || a->token % 32 || a->freq % 32 || a->mlp % H))) {
+  if (a->depth <= 0 || a->depth > DS_MAX_DEPTH || a->n_steps <= 0 || a->n_steps > DS_MAX_STEPS || M > DS_MAXM || 2 * T > 8 ||
+      (head_dim != 64 && head_dim != 96) || H % 8 || a->token % 8 || a->mlp % 8 || a->freq % 8 || bs * T + 1 > DS_MAXM) {
     set_error("dit_ddim_sample: unsupported shape (rows %d <= %d, tokens per sequence <= 8, head_dim = hidden / heads 64 or 96 "
-              "(hidden %lld, heads %lld), dims %% 8; above one sequence also hidden, token, freq %% 32 and mlp %% hidden)", M,
-              maxm, (long long)a->hidden, (long long)a->heads);
+              "(hidden %lld, heads %lld), dims %% 8)", M, DS_MAXM, (long long)a->hidden, (long long)a->heads);
     return DVLA_ERR_UNSUPPORTED;
   }
   if (dvla_dit_sampler_workspace_bytes(a->batch, a->T, a->hidden, a->mlp, a->n_steps) > a->workspace_bytes) {
@@ -622,14 +502,7 @@ extern "C" int dvla_dit_ddim_sample(const dvla_dit_sampler_args* a, void* stream
   int rows = M > bs * T + 1 ? M : bs * T + 1;
   if (p.n_steps > rows) rows = p.n_steps;
   size_t smem = static_cast<size_t>(rows) * widest * 2;
-  size_t xs_bytes = static_cast<size_t>(M) * p.mlp * 2;                // xcur / eps_s sit behind the [M][mlp] staging area
-  if (multi) {                                                         // ... or the widest [rows][K] staged: fc2 runs in K chunks
-    size_t e = static_cast<size_t>(M) * H;
-    if (static_cast<size_t>(bs * T + 1) * p.token > e) e = static_cast<size_t>(bs * T + 1) * p.token;
-    if (static_cast<size_t>(p.n_steps) * (p.freq > H ? p.freq : H) > e) e = static_cast<size_t>(p.n_steps) * (p.freq > H ? p.freq : H);
-    p.xs_elems = static_cast<long long>(e);
-    smem = xs_bytes = e * 2;
-  }
+  const size_t xs_bytes = static_cast<size_t>(M) * p.mlp * 2;          // xcur / eps_s sit behind the [M][mlp] staging area
   if (smem < xs_bytes) smem = xs_bytes;
   smem += static_cast<size_t>(bs * T * C + 2 * bs * T * C) * sizeof(float) + 16;
   if (static_cast<size_t>(bs * T + 1) * p.token * 2 > xs_bytes || static_cast<size_t>(p.n_steps) * (p.freq > H ? p.freq : H) * 2 > xs_bytes) {
@@ -638,7 +511,7 @@ extern "C" int dvla_dit_ddim_sample(const dvla_dit_sampler_args* a, void* stream
   if (smem > 227 * 1024) { set_error("dit_ddim_sample: %zu bytes of shared memory needed", smem); return DVLA_ERR_UNSUPPORTED; }
   if (2 * T != 6) { set_error("dit_ddim_sample: built for action_pred_steps == 3 (6 tokens per sequence), got %d", 2 * T); return DVLA_ERR_UNSUPPORTED; }
   cudaError_t attr_err;
-  void* kern = multi ? sampler_kernel_for<DS_ROWS_TC>(head_dim, fm, &attr_err) : sampler_kernel_for<DS_MAXM>(head_dim, fm, &attr_err);
+  void* kern = sampler_kernel_for(head_dim, fm, &attr_err);
   if (attr_err != cudaSuccess) { set_error("dit_ddim_sample smem attr: %s", cudaGetErrorString(attr_err)); return DVLA_ERR_CUDA; }
   int dev = 0, coop = 0;
   cudaGetDevice(&dev);

@@ -579,16 +579,10 @@ class DreamVLA(nn.Module):
                 and net.x_embedder.linear.weight.shape[0] in (64 * net.num_heads, 96 * net.num_heads)
                 and not torch.is_grad_enabled())
 
-    # Most sequences a batched rollout samples on the fused kernel.  The kernel takes up to 8 (its tensor-core bucket,
-    # csrc/dit_sampler.cu), but on an H100 that bucket is slower than the launch-bound module sampler at every N >= 2
-    # (tools/prof_batched_rollout.py, DESIGN §8), so the measured crossover keeps N >= 2 on the module sampler.
-    FUSED_SAMPLER_MAX_BATCH = 1
-
-    def _ddim_actions(self, feat, sample_noise, dev, multi=False):
-        """10-step DDIM with classifier-free guidance 1.5 (:935-987) on feat [n, action_pred_steps, D] -> [n, steps, 7].
-        multi=True (batched rollouts): the fused kernel takes up to FUSED_SAMPLER_MAX_BATCH sequences."""
+    def _ddim_actions(self, feat, sample_noise, dev):
+        """10-step DDIM with classifier-free guidance 1.5 (:935-987) on feat [n, action_pred_steps, D] -> [n, steps, 7]."""
         bs = feat.shape[0]
-        fused = self._fused_sampler_fits(bs) or (multi and bs <= self.FUSED_SAMPLER_MAX_BATCH and self._fused_sampler_fits(1))
+        fused = self._fused_sampler_fits(bs)
         cfg_scale = 1.5
         if self.use_fm:
             # --use_fm (ActionModelFM / FMDiffusion, respace.py:118-191): the sampler forces the guidance scale to 1.0, ignores
@@ -689,8 +683,8 @@ class DreamVLA(nn.Module):
         text_embedding [N, D], frame_tokens [N, S, 35, D] (window order), sel int32 [N] on the device: every per-env choice --
         mask, token gather, action-row gather -- is made on the device, so one CUDA graph serves every mix of fill levels.
         sample_noise [N, steps, 7] or None.  Returns (arm [N, steps, 6], gripper [N, steps, 1]), or the backbone's action-token
-        rows [N, steps, D] with return_features.  The actions come from the fused sampler kernel up to FUSED_SAMPLER_MAX_BATCH
-        envs (with FUSED_SAMPLER), from the module sampler above (see FUSED_SAMPLER_MAX_BATCH)."""
+        rows [N, steps, D] with return_features.  At N = 1 the actions come from the fused sampler kernel (with
+        FUSED_SAMPLER), at N >= 2 from the module sampler."""
         assert self.use_dit_head and self.action_pred_steps > 0
         N, S = frame_tokens.shape[:2]
         D = self.hidden_dim
@@ -712,7 +706,7 @@ class DreamVLA(nn.Module):
         feat = h.gather(1, arow.unsqueeze(2).expand(N, self.action_pred_steps, D))                 # [N, steps, D]
         if return_features:
             return feat
-        samples = self._ddim_actions(feat, sample_noise, dev, multi=True)
+        samples = self._ddim_actions(feat, sample_noise, dev)
         return samples[..., :6], samples[..., 6:]
 
     @torch.no_grad()

@@ -288,9 +288,8 @@ int dvla_grad_clip_scale(void* g_bf16, int64_t n, const float* sumsq, float max_
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Fused action sampler: the DDIM loop of the DiT action head with classifier-free guidance as ONE persistent cooperative
- * kernel (replaces dreamvla_model.py:935-987 -> gaussian_diffusion.py:609-689 -> models.py:253-268 for small batches).
- * rows = 2 * batch * 2T with 2T = 6: batch 1 (12 rows, FMA GEMMs) or 2 <= batch <= 8 (up to 96 rows, tensor-core GEMMs; hidden,
- * token and freq multiples of 32, mlp a multiple of hidden); a batch above 8 returns DVLA_ERR_UNSUPPORTED before any launch.
+ * kernel (replaces dreamvla_model.py:935-987 -> gaussian_diffusion.py:609-689 -> models.py:253-268 for one sequence).
+ * batch must be 1 (rows = 2 guidance branches * 2T = 12); any other batch returns DVLA_ERR_UNSUPPORTED before any launch.
  * Every pointer is device memory, weights are bf16 nn.Linear layouts [out, in].
  * head_dim = hidden / heads must be 64 (DiT-B, DiT-L) or 96 (DiT-S); DVLA_ERR_UNSUPPORTED otherwise.
  * Schedule tables are HOST arrays of n_steps entries (respaced DDIM: timestep_map[i] is the original timestep of step i).

@@ -94,28 +94,3 @@ def test_negative_mask_stack_strides_are_invalid(lib):
     rc = lib.dvla_attn_fwd(ctypes.byref(a), None)
     assert rc == -1 and b"negative mask_stride" in lib.dvla_last_error()
 
-
-def sampler_args(batch, workspace_bytes=1 << 40):
-    """DiT-B sampler arguments with fake pointers: every call below returns before it launches."""
-    depth, hidden = 12, 768
-    blocks = (_lib.DitBlockWeights * depth)(*[_lib.DitBlockWeights(*[4096 * (i + 1)] * 8) for i in range(depth)])
-    a = _lib.DitSamplerArgs()
-    for n, t in _lib.DitSamplerArgs._fields_:
-        if t is _lib._vp:
-            setattr(a, n, 8192)
-    a.blocks = blocks
-    a.depth, a.hidden, a.heads, a.mlp, a.token, a.freq, a.channels, a.T, a.batch = depth, hidden, 12, 4 * hidden, 1024, 256, 7, 3, batch
-    a.n_steps, a.cfg_scale, a.workspace_bytes = 10, 1.5, workspace_bytes
-    a.timestep_map = (ctypes.c_int32 * 10)(*range(0, 100, 10))
-    for f in ("sqrt_recip_alphas_cumprod", "sqrt_recipm1_alphas_cumprod", "alphas_cumprod_prev"):
-        setattr(a, f, (ctypes.c_float * 10)(*[1.0] * 10))
-    return a
-
-
-def test_fused_sampler_takes_up_to_8_sequences(lib):
-    rc = lib.dvla_dit_ddim_sample(ctypes.byref(sampler_args(9)), None)
-    assert rc == -3 and b"batch 9 outside 1 .. 8" in lib.dvla_last_error()
-    # batch 8 passes every shape check and stops at the (deliberately short) workspace, before any launch
-    need = lib.dvla_dit_sampler_workspace_bytes(8, 3, 768, 3072, 10)
-    rc = lib.dvla_dit_ddim_sample(ctypes.byref(sampler_args(8, workspace_bytes=need - 4)), None)
-    assert rc == -1 and b"workspace too small" in lib.dvla_last_error()

@@ -1,5 +1,6 @@
 """The flow-matching (`--use_fm`) integrator of the fused sampler without a GPU: the C ABI refuses what the kernel does not
-implement on the host, before any launch, and the host's timestep inputs are the module path's fp32 values bit for bit."""
+implement (integrators, step counts, batches other than one sequence) on the host, before any launch, and the host's
+timestep inputs are the module path's fp32 values bit for bit."""
 import ctypes
 import struct
 
@@ -9,7 +10,7 @@ import torch
 DVLA_ERR_INVALID, DVLA_ERR_UNSUPPORTED = -1, -3
 
 
-def _args(integrator, n_steps=10, t_values=True):
+def _args(integrator, n_steps=10, t_values=True, batch=1):
     """A DiT-B-shaped dvla_dit_sampler_args whose device pointers are never dereferenced: every call below is refused by the
     host-side checks."""
     from dreamvla_b200 import _lib as L
@@ -20,7 +21,7 @@ def _args(integrator, n_steps=10, t_values=True):
         if t is L._vp:
             setattr(a, n, 8192)
     a.blocks = blocks
-    a.depth, a.hidden, a.heads, a.mlp, a.token, a.freq, a.channels, a.T, a.batch = depth, hidden, heads, 4 * hidden, 1024, 256, 7, 3, 1
+    a.depth, a.hidden, a.heads, a.mlp, a.token, a.freq, a.channels, a.T, a.batch = depth, hidden, heads, 4 * hidden, 1024, 256, 7, 3, batch
     a.n_steps, a.cfg_scale, a.workspace_bytes = n_steps, 1.0, 1 << 30
     a.integrator = integrator
     if t_values:
@@ -28,7 +29,8 @@ def _args(integrator, n_steps=10, t_values=True):
     return a
 
 
-@pytest.mark.parametrize("case", ["integrator_2", "integrator_-1", "fm_null_t_values", "fm_13_steps", "ddim_13_steps"])
+@pytest.mark.parametrize("case", ["integrator_2", "integrator_-1", "fm_null_t_values", "fm_13_steps", "ddim_13_steps",
+                                  "batch_2", "batch_0"])
 def test_fused_sampler_refuses_on_host(case):
     from dreamvla_b200 import _lib as L
     lib = L.load()
@@ -39,6 +41,10 @@ def test_fused_sampler_refuses_on_host(case):
         "fm_13_steps": (_args(L.DIT_FM_EULER, n_steps=13), DVLA_ERR_UNSUPPORTED, "n_steps 13 above the 12 prologue rows"),
         "ddim_13_steps": (_args(L.DIT_DDIM, n_steps=13, t_values=False), DVLA_ERR_UNSUPPORTED,
                           "n_steps 13 above the 12 prologue rows"),
+        "batch_2": (_args(L.DIT_DDIM, t_values=False, batch=2), DVLA_ERR_UNSUPPORTED,
+                    "batch 2 unsupported: the fused sampler samples one sequence (batch 1)"),
+        "batch_0": (_args(L.DIT_DDIM, t_values=False, batch=0), DVLA_ERR_UNSUPPORTED,
+                    "batch 0 unsupported: the fused sampler samples one sequence (batch 1)"),
     }[case]
     n0 = lib.dvla_launch_count()
     rc = lib.dvla_dit_ddim_sample(ctypes.byref(a), None)

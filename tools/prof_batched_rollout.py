@@ -9,15 +9,13 @@ at N in {1, 2, 4, 8}:
 
   * step: p50 / p99 per batched step and actions/s (N / p50), incremental (`rollout_actions`) and full window (a batch-N
     `mode='test'` forward), CUDA graphs on, envs starting staggered so that a batch mixes window fill levels
-    (`rollout_bench.run_batched`, host clock around each step with a device synchronise on both sides);
-  * sampler: `DreamVLA._ddim_actions` alone on N sequences with CUDA events over many calls -- the module sampler as a CUDA
-    graph replay at every N, the fused kernel (csrc/dit_sampler.cu) at every N -- the measurement behind
-    DreamVLA.FUSED_SAMPLER_MAX_BATCH, the crossover rollouts use; the step rows run with that selection.
+    (`rollout_bench.run_batched`, host clock around each step with a device synchronise on both sides).  The actions of
+    N = 1 come from the fused sampler kernel, those of N >= 2 from the module sampler.
 
 Rounds alternate the models and, within a round, the order of N; each round builds its model afresh.  Medians over rounds are
 reported with their range.  The GPU's name, power limit and SM clocks are read in the same run.
 
-  python tools/prof_batched_rollout.py [--rounds 2] [--steps 40] [--skip 10] [--sampler-iters 30]
+  python tools/prof_batched_rollout.py [--rounds 2] [--steps 40] [--skip 10]
 """
 from __future__ import annotations
 
@@ -61,34 +59,6 @@ def wrapper(name, model, n, mode, dev):
     return BatchedModelWrapper(model, n, history_len=S, gripper_width=True, device=dev, incremental=mode == "incremental")
 
 
-def sampler_ms(model, n, fused, dev, iters):
-    """ms per `_ddim_actions` call on n sequences (fused: the kernel's bucket for n, whatever rollouts select)."""
-    from prof_pretrain import timed
-    model.FUSED_SAMPLER = fused
-    model.FUSED_SAMPLER_MAX_BATCH = 8                  # time the kernel's multi-sequence bucket whatever the selection
-    g = torch.Generator().manual_seed(1)
-    feat = (torch.randn(n, 3, model.hidden_dim, generator=g) * 0.7).to(dev, torch.bfloat16)
-    noise = torch.randn(n, 3, 7, generator=g).to(dev)
-    with torch.no_grad():
-        run = lambda: model._ddim_actions(feat, noise, dev, multi=True)        # noqa: E731
-        for _ in range(3):
-            run()
-        torch.cuda.synchronize()
-        if not fused:
-            graph = torch.cuda.CUDAGraph()
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                run()
-            torch.cuda.current_stream().wait_stream(side)
-            with torch.cuda.graph(graph):
-                run()
-            run = graph.replay
-        run()
-        torch.cuda.synchronize()
-        return timed(run, iters)
-
-
 def round_for(name, dev, r, args):
     from dreamvla_b200.utils import rollout_bench
     model = build(name, dev)
@@ -96,16 +66,11 @@ def round_for(name, dev, r, args):
     out = {}
     for n in (NS if r % 2 == 0 else NS[::-1]):
         for mode in (MODES if r % 2 == 0 else MODES[::-1]):
-            model.FUSED_SAMPLER = True
             w = wrapper(name, model, n, mode, dev)
             lat = rollout_bench.run_batched(w, args.steps, kind, seed=1, episode_len=2 * model.sequence_length + 3)
             out[f"{mode}_n{n}"] = rollout_bench.batched_report(lat, args.skip, n, mode)
             del w
             torch.cuda.empty_cache()
-        for fused in ((True, False) if r % 2 == 0 else (False, True)):
-            out[f"sampler_{'fused' if fused else 'module'}_n{n}_ms"] = sampler_ms(model, n, fused, dev, args.sampler_iters)
-        model.FUSED_SAMPLER_MAX_BATCH = type(model).FUSED_SAMPLER_MAX_BATCH
-    model.FUSED_SAMPLER = True
     del model
     torch.cuda.empty_cache()
     return out
@@ -117,7 +82,6 @@ def main():
     ap.add_argument("--rounds", type=int, default=2)
     ap.add_argument("--steps", type=int, default=40, help="batched steps per model, N, mode and round")
     ap.add_argument("--skip", type=int, default=10, help="leading steps left out of the percentiles (graph capture)")
-    ap.add_argument("--sampler-iters", type=int, default=30)
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("prof_batched_rollout.py needs a GPU")
@@ -146,13 +110,10 @@ def main():
             for mode in MODES:
                 for q in ("p50", "p99", "actions_per_s"):
                     res[m][f"{mode}_n{n}_{q}"], res[m][f"{mode}_n{n}_{q}_range"] = med([x[f"{mode}_n{n}"][q] for x in rounds[m]])
-            for v in ("fused", "module"):
-                res[m][f"sampler_{v}_n{n}_ms"], res[m][f"sampler_{v}_n{n}_range"] = med(
-                    [x[f"sampler_{v}_n{n}_ms"] for x in rounds[m]])
     print(json.dumps({"tool": "prof_batched_rollout", "gpu": info_before.get("name"), "power_limit": info_before.get("power.limit"),
                       "sm_clock_mhz_before": info_before.get("clocks.sm"), "sm_clock_mhz_after": info_after.get("clocks.sm"),
                       "sm_clock_max_mhz": info_before.get("clocks.max.sm"), "steps": args.steps, "skip": args.skip,
-                      "sampler_iters": args.sampler_iters, "rounds": args.rounds, "results": res}))
+                      "rounds": args.rounds, "results": res}))
 
 
 if __name__ == "__main__":
