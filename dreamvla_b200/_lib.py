@@ -536,7 +536,7 @@ def grad_clip_scale(g, sumsq_t, max_norm, grad_scale=1.0):
 
 
 def set_sm_budget(n_sms: int) -> int:
-    """SMs the persistent GEMM kernels size their grids for (0 = all); returns the previous value."""
+    """SMs the persistent GEMM and attention-backward kernels size their grids for (0 = all); returns the previous value."""
     return load().dvla_set_sm_budget(int(n_sms))
 
 

@@ -14,6 +14,7 @@
 // Masking: tile_flags[qt, kt] in {0 skip, 1 partial, 2 full}; partial tiles test bits of mask[i, j/32].
 // Both kernel families share the per-fragment helpers below dropout_bits: mask words, the forward tile step, the dQ-form dS
 // and the scaled bf16 store.  The forward finish and the dK/dV-form P / dS^T stay written out per kernel (see there).
+#include <limits.h>
 #include <string.h>
 
 #include <mutex>
@@ -275,30 +276,40 @@ __device__ __forceinline__ void row_lse_delta(const AttnParams& p, long long bh,
   }
 }
 
-// dS = P o (dP - delta) over the key tile [k0, k0 + 64), rows = queries from row0 with their row_lse_delta: P recomputed
-// from the LSE and sc, dP dropped with the forward's mask.  Leaves dS in s.
-__device__ __forceinline__ void dq_form_ds(const AttnParams& p, float sc, long long bh, int row0, int k0, int flag,
-                                           const float (&lse2)[2], const float (&dlt)[2], float (&s)[8][4],
-                                           const float (&dp)[8][4]) {
+// The mask words and dropout keep bits of this thread's query rows over the key tile [k0, k0 + 64), as dq_ds_cols reads them.
+struct DqTileBits { uint32_t w[2][2], keep[8]; };
+__device__ __forceinline__ void dq_tile_bits(const AttnParams& p, long long bh, int row0, int k0, int flag, DqTileBits& tb) {
+  row_mask_words(p, p.mask, row0, k0, flag, tb.w);
+  if (p.drop_scale != 0.f) dropout_bits(p, bh, row0, k0, false, tb.keep);
+}
+// dS = P o (dP - delta) in fragment columns [t0, t1) of the key tile [k0, k0 + 64), rows = queries with their
+// row_lse_delta: P recomputed from the LSE and sc, dP dropped with the forward's mask.  Leaves dS in s.
+__device__ __forceinline__ void dq_ds_cols(const AttnParams& p, float sc, int k0, const float (&lse2)[2],
+                                           const float (&dlt)[2], const DqTileBits& tb, float (&s)[8][4],
+                                           const float (&dp)[8][4], int t0, int t1) {
   const int c = threadIdx.x & 3;
-  uint32_t w[2][2];
-  row_mask_words(p, p.mask, row0, k0, flag, w);
-  uint32_t keep[8];
-  if (p.drop_scale != 0.f) dropout_bits(p, bh, row0, k0, false, keep);
 #pragma unroll
-  for (int t = 0; t < 8; ++t) {
+  for (int t = t0; t < t1; ++t) {
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
       const int r = e >> 1;
       const int kk = t * 8 + 2 * c + (e & 1);
-      bool vis = (k0 + kk < p.Lk);
-      if (flag == 1) vis = vis && ((w[r][kk >> 5] >> (kk & 31)) & 1u);
-      const float pv = vis ? exp2f(s[t][e] * sc - lse2[r]) : 0.f;
+      // tb.w is all ones outside partial tiles; a hidden key's exponent is -inf, so P is +0 without a branch
+      const bool vis = (k0 + kk < p.Lk) && ((tb.w[r][kk >> 5] >> (kk & 31)) & 1u);
+      const float pv = exp2f(vis ? s[t][e] * sc - lse2[r] : -INFINITY);
       float dpv = dp[t][e];
-      if (p.drop_scale != 0.f) dpv = ((keep[t] >> e) & 1u) ? dpv * p.drop_scale : 0.f;
+      if (p.drop_scale != 0.f) dpv = ((tb.keep[t] >> e) & 1u) ? dpv * p.drop_scale : 0.f;
       s[t][e] = pv * (dpv - dlt[r]);
     }
   }
+}
+// dq_ds_cols over the whole key tile.
+__device__ __forceinline__ void dq_form_ds(const AttnParams& p, float sc, long long bh, int row0, int k0, int flag,
+                                           const float (&lse2)[2], const float (&dlt)[2], float (&s)[8][4],
+                                           const float (&dp)[8][4]) {
+  DqTileBits tb;
+  dq_tile_bits(p, bh, row0, k0, flag, tb);
+  dq_ds_cols(p, sc, k0, lse2, dlt, tb, s, dp, 0, 8);
 }
 
 // Rows row0 + lane/4 + {0, 8} of a fragment times `scale`, as bf16 at dst + row * ss; rows >= L are not stored.
@@ -728,17 +739,21 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(const AttnParams p) {
 // ============================================ backward, wgmma + TMA ================================================
 // Warp-specialised backward for sequences of >= 96 on both sides, in the S^T / dP^T formulation of attn_bwd_dkv_kernel and
 // the S / dP one of attn_bwd_dq_kernel (dq_form_ds):
-//   DKV = true : CTA = key tiles 2x, 2x+1 of one (b, h); consumer group g owns key tile 2x+g (K, V loaded once) and streams
-//                query tiles (Q, dO): S^T = K Q^T, dP^T = V dO^T (wgmma, smem x smem), dV += P^T dO, dK += dS^T Q (wgmma,
-//                register A operand, Q / dO read MN-major)
-//   DKV = false: CTA = query tiles 2x, 2x+1; group g owns query tile 2x+g (Q, dO) and streams key tiles (K, V):
+//   DKV = true : unit = key tiles 2z, 2z+1 of one (b, h); consumer group g owns key tile 2z+g (K, V loaded once) and
+//                streams query tiles (Q, dO): S^T = K Q^T, dP^T = V dO^T (wgmma, smem x smem), dV += P^T dO,
+//                dK += dS^T Q (wgmma, register A operand, Q / dO read MN-major)
+//   DKV = false: unit = query tiles 2z, 2z+1; group g owns query tile 2z+g (Q, dO) and streams key tiles (K, V):
 //                S = Q K^T, dP = dO V^T, dQ += dS K
-// Warpgroup 2 is the producer (3-stage ring of streamed tile pairs); a streamed tile is loaded when either group sees it.
-// Its thread 0 issues the TMA loads.  In the dK/dV kernel all 128 of its threads also fill the stage's row statistics
-// (below) before they arrive on the stage's full barrier, so the consumers read each query's lse, delta, mask word and
-// dropout keep bits with one shared load per two queries instead of per element.  setmaxnreg hands the producer's
-// registers to the consumers, which hold dK, dV, S^T and dP^T (128 x 56 + 256 x 224 registers <= 64 K; at 40 the
-// producer's Philox draws spill).
+// The grid is persistent: CTA c runs units c, c + grid, c + 2 grid, ... (wb_unit gives their order).  Warpgroup 2 is the
+// producer: it loads each unit's fixed tiles into one of two buffers and streams the unit's tile pairs through a 3-stage
+// ring that carries on across units, so the next unit's fixed tiles and first streamed stages arrive while the consumers
+// finish the current one and store its gradients.  A streamed tile is loaded when either group sees it; its thread 0
+// issues the TMA loads.  In the dK/dV kernel all 128 of its threads also fill the stage's row statistics (below) before
+// they arrive on the stage's full barrier, so the consumers read each query's lse, delta, mask word and dropout keep bits
+// with one shared load per two queries instead of per element.  setmaxnreg hands the producer's registers to the
+// consumers, which hold dK, dV, S^T and dP^T (128 x 64 + 256 x 216 registers within the 384 x 168 of the launch; at 56
+// the producer's Philox draws spill beside the unit it walks).  The consumers issue each k-step of the dV / dK / dQ
+// MMAs as soon as its 16 columns of P and dS are formed, so those MMAs run under the rest of the element-wise pass.
 struct WgmmaBwdMaps { CUtensorMap f0, f1, s0, s1; int f0_hi, f1_hi, s0_hi, s1_hi; };
 constexpr int WB_THREADS = 384;
 // Row statistics of one stage's query tile, in 32-bit words: lse * log2(e) and delta of its 64 queries (+inf and 0 past
@@ -746,28 +761,45 @@ constexpr int WB_THREADS = 384;
 // dropout keep bits.  Keep word ww of a query packs its 8-key Philox blocks 4 ww .. 4 ww + 3, the forward's blocks, so
 // bit (key & 31) of word key / 32 is the key's keep bit, as in the mask.
 constexpr int WB_STAT_LSE = 0, WB_STAT_DELTA = 64, WB_STAT_MASK = 128, WB_STAT_KEEP = 384, WB_STAT_WORDS = 640;
+constexpr int WB_FIXED_BYTES = 4 * 8192;                  // one unit's fixed tiles: [group][f0 8 KB | f1 8 KB]
+
+// Unit u = (z * B + b) * H + h: fixed tile pair z of (b, h).  Every (b, h) runs its heaviest pair before any lighter one
+// across the whole grid: under block-causal masks early key tiles are seen by the most queries and late query tiles see
+// the most keys, so z counts up from the first key pair (dK/dV) or down from the last query pair (dQ).
+struct WbUnit { int b, h, ft_base; };
+__host__ __device__ inline WbUnit wb_unit(bool dkv, int u, int B, int H, int nf) {
+  const int nfb = (nf + 1) / 2;
+  const int h = u % H, r = u / H, b = r % B, z = r / B;
+  return {b, h, 2 * (dkv ? z : nfb - 1 - z)};
+}
 
 template <bool DKV>
 // One CTA per SM: dK and dV accumulators next to S and dP need ~160 registers.
 __global__ void __launch_bounds__(WB_THREADS, 1) attn_bwd_wgmma_kernel(const __grid_constant__ WgmmaBwdMaps tm, const AttnParams p) {
   extern __shared__ uint8_t wb_smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(wb_smem_raw) + 1023) & ~uintptr_t(1023));
-  const uint32_t sF = smem_u32(smem);                       // [group][f0 8 KB | f1 8 KB]
-  const uint32_t sS = sF + 4 * 8192;                        // [stage][s0 8 KB | s1 8 KB]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 4 * 8192 + WF_STAGES * 2 * 8192);
-  uint64_t* f_full = bars;
-  uint64_t* full = bars + 1;
+  // offset from the __shared__ array itself, so that the compiler sees shared-memory accesses (LDS / STS, not generic)
+  uint8_t* smem = wb_smem_raw + ((1024 - (smem_u32(wb_smem_raw) & 1023)) & 1023);
+  const uint32_t sF = smem_u32(smem);                       // [buffer][group][f0 8 KB | f1 8 KB]
+  const uint32_t sS = sF + 2 * WB_FIXED_BYTES;              // [stage][s0 8 KB | s1 8 KB]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 2 * WB_FIXED_BYTES + WF_STAGES * 2 * 8192);
+  uint64_t* f_full = bars;                                  // [buffer]
+  uint64_t* f_empty = bars + 2;                             // [buffer]
+  uint64_t* full = bars + 4;
   uint64_t* empty = full + WF_STAGES;
-  uint32_t* stats = reinterpret_cast<uint32_t*>(smem + 4 * 8192 + WF_STAGES * 2 * 8192 + 128);   // [stage][WB_STAT_WORDS]
-  const int h = blockIdx.x, b = blockIdx.y;
+  uint32_t* stats = reinterpret_cast<uint32_t*>(smem + 2 * WB_FIXED_BYTES + WF_STAGES * 2 * 8192 + 128);   // [stage][WB_STAT_WORDS]
   const int nf = DKV ? p.nkt : p.nqt;                       // tiles on the fixed side
   const int ns = DKV ? p.nqt : p.nkt;                       // tiles on the streamed side
-  const int nfb = (nf + 1) / 2;
-  // heaviest blocks first under block-causal masks: early key tiles are seen by the most queries, late query tiles see
-  // the most keys; blockIdx.z is the slowest launch dimension, so every (b, h) starts its heavy blocks before any light one
-  const int ft_base = 2 * (DKV ? static_cast<int>(blockIdx.z) : nfb - 1 - static_cast<int>(blockIdx.z));
-  const bool has1 = ft_base + 1 < nf;
+  const int units = (nf + 1) / 2 * p.B * p.H;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  int h = 0, b = 0, ft_base = 0;                            // the current unit
+  bool has1 = false;
+  int bh = 0;                                               // b * H + h
+  auto set_unit = [&](int u) {
+    const WbUnit w = wb_unit(DKV, u, p.B, p.H, nf);
+    h = w.h; b = w.b; ft_base = w.ft_base;
+    has1 = ft_base + 1 < nf;
+    bh = b * p.H + h;
+  };
   auto flag_of = [&](int st_, int g) -> int {               // tile flag of (fixed tile ft_base+g, streamed tile st_)
     if (g == 1 && !has1) return 0;
     if (!p.tile_flags) return 2;
@@ -780,177 +812,207 @@ __global__ void __launch_bounds__(WB_THREADS, 1) attn_bwd_wgmma_kernel(const __g
   };
 
   if (threadIdx.x == 0) {
-    mbar_init(f_full, 1);
+    for (int i = 0; i < 2; ++i) { mbar_init(&f_full[i], 1); mbar_init(&f_empty[i], 8); }
     // dK/dV: the TMA thread's expect_tx arrival and one arrival per producer thread once its statistics are written
     for (int st = 0; st < WF_STAGES; ++st) { mbar_init(&full[st], DKV ? 1 + 128 : 1); mbar_init(&empty[st], 8); }
     fence_barrier_init();
   }
   __syncthreads();
-  const long long bh = static_cast<long long>(b) * p.H + h;
 
   if (warp >= 8) {
-    setmaxnreg_dec<56>();
+    setmaxnreg_dec<64>();
     const int pt = threadIdx.x - 256;
     if (!DKV && pt != 0) return;
-    if (pt == 0) {
-      tma_prefetch_desc(&tm.f0); tma_prefetch_desc(&tm.f1); tma_prefetch_desc(&tm.s0); tma_prefetch_desc(&tm.s1);
-      mbar_expect_tx(f_full, 4 * 8192);
-      for (int g = 0; g < 2; ++g) {                         // a tile past the sequence end is zero-filled
-        tma_rows(sF + g * 16384, &tm.f0, f_full, tm.f0_hi, (ft_base + g) * 64, h, b);
-        tma_rows(sF + g * 16384 + 8192, &tm.f1, f_full, tm.f1_hi, (ft_base + g) * 64, h, b);
-      }
-    }
+    if (pt == 0) { tma_prefetch_desc(&tm.f0); tma_prefetch_desc(&tm.f1); tma_prefetch_desc(&tm.s0); tma_prefetch_desc(&tm.s1); }
     const uint64_t seed = p.drop_seed + (p.drop_seed_ptr ? __ldg(p.drop_seed_ptr) : 0ull);
     const int nblk = (p.Lk + 7) >> 3;
     int st = 0; uint32_t ph = 0;
-    for (int t = next_tile(0); t < ns; t = next_tile(t + 1)) {
-      mbar_wait<false>(&empty[st], ph ^ 1);
-      if (pt == 0) {
-        mbar_expect_tx(&full[st], 2 * 8192);
-        tma_rows(sS + st * 16384, &tm.s0, &full[st], tm.s0_hi, t * 64, h, b);
-        tma_rows(sS + st * 16384 + 8192, &tm.s1, &full[st], tm.s1_hi, t * 64, h, b);
-      }
-      if (DKV) {
-        // thread pt: lse (pt < 64) or delta (pt >= 64) of query pt % 64; mask and keep words of query pt % 64 for
-        // consumer group pt / 64, written only where that group reads them (flag 1 / flag != 0 with dropout)
-        uint32_t* sw = stats + st * WB_STAT_WORDS;
-        const int qc = pt & 63, gg = pt >> 6;
-        const int qi = t * 64 + qc;
-        const bool qin = qi < p.Lq;
-        if (pt < 64) reinterpret_cast<float*>(sw)[WB_STAT_LSE + qc] = qin ? p.lse[bh * p.Lq + qi] * LOG2E : INFINITY;
-        else         reinterpret_cast<float*>(sw)[WB_STAT_DELTA + qc] = qin ? p.delta[bh * p.Lq + qi] : 0.f;
-        const int flag = flag_of(t, gg);
-        const int kb0 = (ft_base + gg) * 8;                 // first 8-key block of the group's key tile
-#pragma unroll
-        for (int ww = 0; ww < 2; ++ww) {
-          const int slot = (gg * 2 + ww) * 64 + qc;
-          if (flag == 1) {
-            const int wi = (kb0 >> 2) + ww;
-            sw[WB_STAT_MASK + slot] = (qin && wi < p.mask_words) ? __ldg(p.mask + static_cast<long long>(qi) * p.mask_words + wi) : 0u;
-          }
-          if (flag != 0 && p.drop_scale != 0.f) {
-            uint32_t kw = 0;
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-              kw |= dropout_keep8(seed, (bh * p.Lq + qi) * nblk + kb0 + ww * 4 + j, p.drop_thresh) << (8 * j);
-            sw[WB_STAT_KEEP + slot] = kw;
-          }
+    for (int u = blockIdx.x; u < units; u += gridDim.x) {
+      set_unit(u);
+      if (pt == 0) {                                        // fixed buffer i % 2, free once unit i - 2 is done with it
+        const int i = (u - blockIdx.x) / gridDim.x;         // the CTA's unit count, not carried: the producer's
+        const int fb = i & 1;                               // registers are tight around the Philox draws
+        mbar_wait<false>(&f_empty[fb], ((i >> 1) & 1) ^ 1);
+        mbar_expect_tx(&f_full[fb], WB_FIXED_BYTES);
+        const uint32_t dst = sF + fb * WB_FIXED_BYTES;
+        for (int g = 0; g < 2; ++g) {                       // a tile past the sequence end is zero-filled
+          tma_rows(dst + g * 16384, &tm.f0, &f_full[fb], tm.f0_hi, (ft_base + g) * 64, h, b);
+          tma_rows(dst + g * 16384 + 8192, &tm.f1, &f_full[fb], tm.f1_hi, (ft_base + g) * 64, h, b);
         }
-        mbar_arrive(&full[st]);
       }
-      if (++st == WF_STAGES) { st = 0; ph ^= 1; }
+      for (int t = next_tile(0); t < ns; t = next_tile(t + 1)) {
+        mbar_wait<false>(&empty[st], ph ^ 1);
+        if (pt == 0) {
+          mbar_expect_tx(&full[st], 2 * 8192);
+          tma_rows(sS + st * 16384, &tm.s0, &full[st], tm.s0_hi, t * 64, h, b);
+          tma_rows(sS + st * 16384 + 8192, &tm.s1, &full[st], tm.s1_hi, t * 64, h, b);
+        }
+        if (DKV) {
+          // thread pt: lse (pt < 64) or delta (pt >= 64) of query pt % 64; mask and keep words of query pt % 64 for
+          // consumer group pt / 64, written only where that group reads them (flag 1 / flag != 0 with dropout)
+          uint32_t* sw = stats + st * WB_STAT_WORDS;
+          const int qc = pt & 63, gg = pt >> 6;
+          const int qi = t * 64 + qc;
+          const bool qin = qi < p.Lq;
+          if (pt < 64) reinterpret_cast<float*>(sw)[WB_STAT_LSE + qc] = qin ? p.lse[static_cast<long long>(bh) * p.Lq + qi] * LOG2E : INFINITY;
+          else         reinterpret_cast<float*>(sw)[WB_STAT_DELTA + qc] = qin ? p.delta[static_cast<long long>(bh) * p.Lq + qi] : 0.f;
+          const int flag = flag_of(t, gg);
+          const int kb0 = (ft_base + gg) * 8;               // first 8-key block of the group's key tile
+#pragma unroll
+          for (int ww = 0; ww < 2; ++ww) {
+            const int slot = (gg * 2 + ww) * 64 + qc;
+            if (flag == 1) {
+              const int wi = (kb0 >> 2) + ww;
+              sw[WB_STAT_MASK + slot] = (qin && wi < p.mask_words) ? __ldg(p.mask + static_cast<long long>(qi) * p.mask_words + wi) : 0u;
+            }
+            if (flag != 0 && p.drop_scale != 0.f) {
+              uint32_t kw = 0;
+#pragma unroll
+              for (int j = 0; j < 4; ++j)
+                kw |= dropout_keep8(seed, (static_cast<long long>(bh) * p.Lq + qi) * nblk + kb0 + ww * 4 + j, p.drop_thresh) << (8 * j);
+              sw[WB_STAT_KEEP + slot] = kw;
+            }
+          }
+          mbar_arrive(&full[st]);
+        }
+        if (++st == WF_STAGES) { st = 0; ph ^= 1; }
+      }
     }
     return;
   }
 
-  setmaxnreg_inc<224>();
+  setmaxnreg_inc<216>();
   const int g = warp >> 2, wq = warp & 3;
   const int c = lane & 3, gr = lane >> 2;
-  const int f0 = (ft_base + g) * 64;                        // first key (DKV) / query (dQ) row of this group
   const float sc = p.scale * LOG2E;
-  const uint32_t fa0 = sF + g * 16384, fa1 = fa0 + 8192;   // DKV: K, V of the key tile; dQ: Q, dO of the query tile
-  float acc0[8][4], acc1[8][4];                             // DKV: dK, dV; dQ: dQ (acc1 unused)
-  zero_c(acc0);
-  zero_c(acc1);
-  float lse2[2], dlt[2];
-  if (!DKV) row_lse_delta(p, bh, f0 + wq * 16, lse2, dlt);
-  mbar_wait<false>(f_full, 0);
-
   int st = 0; uint32_t ph = 0;
-  for (int t = next_tile(0); t < ns; t = next_tile(t + 1)) {
-    mbar_wait<false>(&full[st], ph);
-    const int flag = flag_of(t, g);
-    if (flag != 0) {
+  for (int u = blockIdx.x, i = 0; u < units; u += gridDim.x, ++i) {
+    set_unit(u);
+    const int fb = i & 1;
+    const int f0 = (ft_base + g) * 64;                      // first key (DKV) / query (dQ) row of this group
+    const uint32_t fa0 = sF + fb * WB_FIXED_BYTES + g * 16384, fa1 = fa0 + 8192;   // DKV: K, V of the key tile; dQ: Q, dO
+    float acc0[8][4], acc1[8][4];                           // DKV: dK, dV; dQ: dQ (acc1 unused)
+    zero_c(acc0);
+    zero_c(acc1);
+    float lse2[2], dlt[2];
+    if (!DKV) row_lse_delta(p, bh, f0 + wq * 16, lse2, dlt);
+    mbar_wait<false>(&f_full[fb], (i >> 1) & 1);
+
+    for (int t = next_tile(0); t < ns; t = next_tile(t + 1)) {
+      mbar_wait<false>(&full[st], ph);
+      const int flag = flag_of(t, g);
       const uint32_t sa0 = sS + st * 16384, sa1 = sa0 + 8192;   // DKV: Q, dO of the query tile; dQ: K, V of the key tile
-      const int s0r = t * 64;
       float s[8][4], dp[8][4];
       float (&sd)[32] = *reinterpret_cast<float(*)[32]>(&s[0][0]);
       float (&dpd)[32] = *reinterpret_cast<float(*)[32]>(&dp[0][0]);
-      wgmma_fence();
+      if (flag != 0) {
+        wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < 4; ++k)
-        wgmma_m64n64k16_ss(sd, make_smem_desc_sw128(fa0 + k * 32, 16, 1024), make_smem_desc_sw128(sa0 + k * 32, 16, 1024), k != 0);
+        for (int k = 0; k < 4; ++k)
+          wgmma_m64n64k16_ss(sd, make_smem_desc_sw128(fa0 + k * 32, 16, 1024), make_smem_desc_sw128(sa0 + k * 32, 16, 1024), k != 0);
 #pragma unroll
-      for (int k = 0; k < 4; ++k)
-        wgmma_m64n64k16_ss(dpd, make_smem_desc_sw128(fa1 + k * 32, 16, 1024), make_smem_desc_sw128(sa1 + k * 32, 16, 1024), k != 0);
-      wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_operand32(sd);
-      wgmma_fence_operand32(dpd);
-      if (DKV) {
-        // ---- as attn_bwd_dkv_kernel: rows = keys (f0 + ...), cols = queries (s0r + ...), with the query's lse, delta,
-        // mask word and keep bits from the stage's statistics (the producer wrote them before the full barrier) ----
-        const int k0 = f0;
-        const uint32_t* sw = stats + st * WB_STAT_WORDS;
-        const int slot = (g * 2 + (wq >> 1)) * 64;            // mask / keep word of this warp's 16 key rows
-        float pt[8][4];
+        for (int k = 0; k < 4; ++k)
+          wgmma_m64n64k16_ss(dpd, make_smem_desc_sw128(fa1 + k * 32, 16, 1024), make_smem_desc_sw128(sa1 + k * 32, 16, 1024), k != 0);
+        wgmma_commit();
+        const int s0r = t * 64;
+        wgmma_wait<0>();
+        wgmma_fence_operand32(sd);
+        wgmma_fence_operand32(dpd);
+        if (DKV) {
+          // ---- as attn_bwd_dkv_kernel: rows = keys (f0 + ...), cols = queries (s0r + ...), with the query's lse, delta,
+          // mask word and keep bits from the stage's statistics (the producer wrote them before the full barrier) ----
+          const int k0 = f0;
+          const uint32_t* sw = stats + st * WB_STAT_WORDS;
+          const int slot = (g * 2 + (wq >> 1)) * 64;            // mask / keep word of this warp's 16 key rows
+          float pt[8][4];
+          uint32_t pa[4][4], da[4][4];
+          float (&dkd)[32] = *reinterpret_cast<float(*)[32]>(&acc0[0][0]);
+          float (&dvd)[32] = *reinterpret_cast<float(*)[32]>(&acc1[0][0]);
+          // 16 queries at a time: their P^T and dS^T columns are the A operand of k-step kk of dV += P^T dO and
+          // dK += dS^T Q, issued as soon as they are formed so the MMAs run under the next columns' element-wise pass.
+          // Each accumulator still takes its k-steps in order.
 #pragma unroll
-        for (int tt = 0; tt < 8; ++tt) {
-          const int qc = tt * 8 + 2 * c;                      // this thread's queries qc, qc + 1 of the tile
-          const float2 lse_q = *reinterpret_cast<const float2*>(sw + WB_STAT_LSE + qc);
-          const float2 dlt_q = *reinterpret_cast<const float2*>(sw + WB_STAT_DELTA + qc);
-          uint2 mw = make_uint2(0u, 0u), kw = make_uint2(0u, 0u);
-          if (flag == 1) mw = *reinterpret_cast<const uint2*>(sw + WB_STAT_MASK + slot + qc);
-          if (p.drop_scale != 0.f) kw = *reinterpret_cast<const uint2*>(sw + WB_STAT_KEEP + slot + qc);
+          for (int kk = 0; kk < 4; ++kk) {
 #pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const int kr = wq * 16 + gr + (e >> 1) * 8;
-            const float lse_e = (e & 1) ? lse_q.y : lse_q.x, dlt_e = (e & 1) ? dlt_q.y : dlt_q.x;
-            bool vis = (k0 + kr < p.Lk);
-            if (flag == 1) vis = vis && ((((e & 1) ? mw.y : mw.x) >> (kr & 31)) & 1u);
-            const float pv = vis ? exp2f(s[tt][e] * sc - lse_e) : 0.f;
-            float dpv = dp[tt][e];
-            float pdrop = pv;
-            if (p.drop_scale != 0.f) {
-              const bool kp = ((((e & 1) ? kw.y : kw.x) >> (kr & 31)) & 1u);
-              pdrop = kp ? pv * p.drop_scale : 0.f;
-              dpv = kp ? dpv * p.drop_scale : 0.f;
+            for (int tt = 2 * kk; tt < 2 * kk + 2; ++tt) {
+              const int qc = tt * 8 + 2 * c;                    // this thread's queries qc, qc + 1 of the tile
+              const float2 lse_q = *reinterpret_cast<const float2*>(sw + WB_STAT_LSE + qc);
+              const float2 dlt_q = *reinterpret_cast<const float2*>(sw + WB_STAT_DELTA + qc);
+              uint2 mw = make_uint2(~0u, ~0u), kw = make_uint2(0u, 0u);   // mask words: all ones outside partial tiles
+              if (flag == 1) mw = *reinterpret_cast<const uint2*>(sw + WB_STAT_MASK + slot + qc);
+              if (p.drop_scale != 0.f) kw = *reinterpret_cast<const uint2*>(sw + WB_STAT_KEEP + slot + qc);
+#pragma unroll
+              for (int e = 0; e < 4; ++e) {
+                const int kr = wq * 16 + gr + (e >> 1) * 8;
+                const float lse_e = (e & 1) ? lse_q.y : lse_q.x, dlt_e = (e & 1) ? dlt_q.y : dlt_q.x;
+                // a hidden key's exponent is -inf, so P is +0 without a branch
+                const bool vis = (k0 + kr < p.Lk) && ((((e & 1) ? mw.y : mw.x) >> (kr & 31)) & 1u);
+                const float pv = exp2f(vis ? s[tt][e] * sc - lse_e : -INFINITY);
+                float dpv = dp[tt][e];
+                float pdrop = pv;
+                if (p.drop_scale != 0.f) {
+                  const bool kp = ((((e & 1) ? kw.y : kw.x) >> (kr & 31)) & 1u);
+                  pdrop = kp ? pv * p.drop_scale : 0.f;
+                  dpv = kp ? dpv * p.drop_scale : 0.f;
+                }
+                pt[tt][e] = pdrop;
+                s[tt][e] = pv * (dpv - dlt_e);
+              }
             }
-            pt[tt][e] = pdrop;
-            s[tt][e] = pv * (dpv - dlt_e);
+            pa[kk][0] = pack_bf16x2(pt[2 * kk][0], pt[2 * kk][1]);       // c_to_a, k-step kk
+            pa[kk][1] = pack_bf16x2(pt[2 * kk][2], pt[2 * kk][3]);
+            pa[kk][2] = pack_bf16x2(pt[2 * kk + 1][0], pt[2 * kk + 1][1]);
+            pa[kk][3] = pack_bf16x2(pt[2 * kk + 1][2], pt[2 * kk + 1][3]);
+            da[kk][0] = pack_bf16x2(s[2 * kk][0], s[2 * kk][1]);
+            da[kk][1] = pack_bf16x2(s[2 * kk][2], s[2 * kk][3]);
+            da[kk][2] = pack_bf16x2(s[2 * kk + 1][0], s[2 * kk + 1][1]);
+            da[kk][3] = pack_bf16x2(s[2 * kk + 1][2], s[2 * kk + 1][3]);
+            wgmma_fence();
+            wgmma_m64n64k16_rs_tb(dvd, pa[kk], make_smem_desc_sw128(sa1 + kk * 2048, 8192, 1024));
+            wgmma_m64n64k16_rs_tb(dkd, da[kk], make_smem_desc_sw128(sa0 + kk * 2048, 8192, 1024));
           }
+          wgmma_commit();
+          wgmma_wait<0>();
+          wgmma_fence_operand32(dkd);
+          wgmma_fence_operand32(dvd);
+        } else {
+          // rows = queries (f0 + ...), cols = keys (s0r + ...); k-step kk of dQ += dS K is issued once dS has its 16 keys,
+          // as in the dK/dV kernel
+          DqTileBits tb;
+          dq_tile_bits(p, bh, f0 + wq * 16, s0r, flag, tb);
+          uint32_t da[4][4];
+          float (&dqd)[32] = *reinterpret_cast<float(*)[32]>(&acc0[0][0]);
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk) {
+            dq_ds_cols(p, sc, s0r, lse2, dlt, tb, s, dp, 2 * kk, 2 * kk + 2);
+            da[kk][0] = pack_bf16x2(s[2 * kk][0], s[2 * kk][1]);        // c_to_a, k-step kk
+            da[kk][1] = pack_bf16x2(s[2 * kk][2], s[2 * kk][3]);
+            da[kk][2] = pack_bf16x2(s[2 * kk + 1][0], s[2 * kk + 1][1]);
+            da[kk][3] = pack_bf16x2(s[2 * kk + 1][2], s[2 * kk + 1][3]);
+            wgmma_fence();
+            wgmma_m64n64k16_rs_tb(dqd, da[kk], make_smem_desc_sw128(sa0 + kk * 2048, 8192, 1024));
+          }
+          wgmma_commit();
+          wgmma_wait<0>();
+          wgmma_fence_operand32(dqd);
         }
-        uint32_t pa[4][4], da[4][4];
-        c_to_a(pt, pa);
-        c_to_a(s, da);
-        float (&dkd)[32] = *reinterpret_cast<float(*)[32]>(&acc0[0][0]);
-        float (&dvd)[32] = *reinterpret_cast<float(*)[32]>(&acc1[0][0]);
-        wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) wgmma_m64n64k16_rs_tb(dvd, pa[kk], make_smem_desc_sw128(sa1 + kk * 2048, 8192, 1024));
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) wgmma_m64n64k16_rs_tb(dkd, da[kk], make_smem_desc_sw128(sa0 + kk * 2048, 8192, 1024));
-        wgmma_commit();
-        wgmma_wait<0>();
-        wgmma_fence_operand32(dkd);
-        wgmma_fence_operand32(dvd);
-      } else {
-        // rows = queries (f0 + ...), cols = keys (s0r + ...)
-        dq_form_ds(p, sc, bh, f0 + wq * 16, s0r, flag, lse2, dlt, s, dp);
-        uint32_t da[4][4];
-        c_to_a(s, da);
-        float (&dqd)[32] = *reinterpret_cast<float(*)[32]>(&acc0[0][0]);
-        wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) wgmma_m64n64k16_rs_tb(dqd, da[kk], make_smem_desc_sw128(sa0 + kk * 2048, 8192, 1024));
-        wgmma_commit();
-        wgmma_wait<0>();
-        wgmma_fence_operand32(dqd);
       }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[st]);
+      if (++st == WF_STAGES) { st = 0; ph ^= 1; }
     }
     __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[st]);
-    if (++st == WF_STAGES) { st = 0; ph ^= 1; }
-  }
-  if (g == 1 && !has1) return;
-  if (DKV) {
-    store_frag_bf16(p.dk + b * p.dk_sb + h * p.dk_sh, p.dk_ss, f0 + wq * 16, p.Lk, acc0, p.scale);
-    store_frag_bf16(p.dv + b * p.dv_sb + h * p.dv_sh, p.dv_ss, f0 + wq * 16, p.Lk, acc1, 1.f);
-  } else {
-    store_frag_bf16(p.dq + b * p.dq_sb + h * p.dq_sh, p.dq_ss, f0 + wq * 16, p.Lq, acc0, p.scale);
+    if (lane == 0) mbar_arrive(&f_empty[fb]);               // the fixed tiles are read by the S/dP MMAs only
+    if (g == 1 && !has1) continue;
+    if (DKV) {
+      store_frag_bf16(p.dk + b * p.dk_sb + h * p.dk_sh, p.dk_ss, f0 + wq * 16, p.Lk, acc0, p.scale);
+      store_frag_bf16(p.dv + b * p.dv_sb + h * p.dv_sh, p.dv_ss, f0 + wq * 16, p.Lk, acc1, 1.f);
+    } else {
+      store_frag_bf16(p.dq + b * p.dq_sb + h * p.dq_sh, p.dq_ss, f0 + wq * 16, p.Lq, acc0, p.scale);
+    }
   }
 }
-constexpr int WB_SMEM = 1024 + 4 * 8192 + WF_STAGES * 2 * 8192 + 128 + WF_STAGES * WB_STAT_WORDS * 4;
+constexpr int WB_SMEM = 1024 + 2 * WB_FIXED_BYTES + WF_STAGES * 2 * 8192 + 128 + WF_STAGES * WB_STAT_WORDS * 4;
 
 // ===================================================== mask tiles =================================================
 __global__ void attn_mask_tiles_kernel(const uint32_t* __restrict__ mask, int mask_words, int Lq, int Lk, int nkt,
@@ -1087,7 +1149,10 @@ static int attn_bwd_wgmma_launch(const WgmmaBwdMaps& tm, const AttnParams& p, cu
   static cudaError_t attr_err = cudaSuccess;
   if (!set_smem_attr_once(once, attr_err, attn_bwd_wgmma_kernel<DKV>, WB_SMEM)) { set_error("attn_bwd_wgmma smem attribute: %s", cudaGetErrorString(attr_err)); return DVLA_ERR_CUDA; }
   const int nf = DKV ? p.nkt : p.nqt;
-  attn_bwd_wgmma_kernel<DKV><<<dim3(p.H, p.B, (nf + 1) / 2), WB_THREADS, WB_SMEM, s>>>(tm, p);
+  const long long units = (long long)(nf + 1) / 2 * p.B * p.H;
+  if (units > INT_MAX) { set_error("attn_bwd_wgmma: %lld work units exceed the int index", units); return DVLA_ERR_UNSUPPORTED; }
+  const int grid = units < num_sms() ? (int)units : num_sms();   // persistent: one CTA per SM the budget leaves us
+  attn_bwd_wgmma_kernel<DKV><<<grid, WB_THREADS, WB_SMEM, s>>>(tm, p);
   DVLA_CHECK_LAUNCH(DKV ? "attn_bwd_dkv_wgmma" : "attn_bwd_dq_wgmma");
   return DVLA_OK;
 }

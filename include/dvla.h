@@ -381,9 +381,10 @@ int dvla_image_fn(const dvla_image_fn_args* args, void* stream);
 int32_t dvla_bicubic_taps(int64_t in_size, int64_t out_size);
 int dvla_bicubic_coeffs(int64_t in_size, int64_t out_size, int64_t first, int64_t count, int32_t* bounds, int32_t* coeffs);
 
-/* SM budget of the persistent GEMM kernels (one CTA / CTA pair per SM).  0 = all SMs (default).  The data-parallel train
- * step lowers it by the number of CTAs the NCCL all-reduce occupies while gradient exchange overlaps the backward pass
- * (train.py:173 DDP overlap), so that every GEMM CTA is resident at once.  Returns the previous value.  Process-wide. */
+/* SM budget of the persistent GEMM and attention-backward kernels (one CTA / CTA pair per SM).  0 = all SMs (default).
+ * The data-parallel train step lowers it by the number of CTAs the NCCL all-reduce occupies while gradient exchange
+ * overlaps the backward pass (train.py:173 DDP overlap), so that every persistent CTA is resident at once.  Returns the
+ * previous value.  Process-wide. */
 int dvla_set_sm_budget(int n_sms);
 
 /* ---------------------------------------------------------------------------------------------------------------
