@@ -216,9 +216,24 @@ def gemm_workspace(device):
     return ws
 
 
-def gemm(a, b, *, a_mn=False, b_mn=False, bias=None, act=0, residual=None, aux_out=None, aux_in=None, out=None,
-         out_dtype=torch.bfloat16, alpha=1.0, dropout_p=0.0, dropout_seed=0, dropout_seed_ptr=None):
-    """out[M,N] = epi(alpha * A @ B^T).  a: [M,K] (or [K,M] if a_mn), b: [N,K] (or [K,N] if b_mn); 2-D, unit inner stride."""
+def gemm(a, b, **kw):
+    """out[M,N] = epi(alpha * A @ B^T).  a: [M,K] (or [K,M] if a_mn), b: [N,K] (or [K,N] if b_mn); 2-D, unit inner stride.
+    Keywords: see _gemm_args."""
+    args, out = _gemm_args(a, b, **kw)
+    _call("dvla_gemm", C.byref(args), _stream())
+    return out
+
+
+def gemm_plan(a, b, **kw) -> GemmPlanInfo:
+    """What gemm(a, b, **kw) would launch on the current device (dvla_gemm_plan of the same arguments); launches nothing."""
+    args, _ = _gemm_args(a, b, **kw)
+    info = GemmPlanInfo()
+    _call("dvla_gemm_plan", C.byref(args), C.byref(info))
+    return info
+
+
+def _gemm_args(a, b, *, a_mn=False, b_mn=False, bias=None, act=0, residual=None, aux_out=None, aux_in=None, out=None,
+               out_dtype=torch.bfloat16, alpha=1.0, dropout_p=0.0, dropout_seed=0, dropout_seed_ptr=None):
     _need_cuda(a, b)
     assert a.dim() == 2 and b.dim() == 2 and a.stride(1) == 1 and b.stride(1) == 1, (a.shape, a.stride(), b.shape, b.stride())
     assert a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16
@@ -251,8 +266,7 @@ def gemm(a, b, *, a_mn=False, b_mn=False, bias=None, act=0, residual=None, aux_o
     args.dropout_seed_ptr = _ptr(dropout_seed_ptr)
     ws = gemm_workspace(a.device)
     args.workspace, args.workspace_bytes = ws.data_ptr(), ws.numel()
-    _call("dvla_gemm", C.byref(args), _stream())
-    return out
+    return args, out
 
 
 def layernorm_fwd(x2d, gamma, beta, eps, save_stats=True):

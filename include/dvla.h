@@ -67,8 +67,9 @@ typedef struct {
   /* optional scratch of >= dvla_gemm_workspace_bytes() bytes, 16-byte aligned, owned by one stream (calls on one stream may
    * share it).  Its first 64 KB are arrival counters: ZERO before the first call, left zero by every call; the rest holds
    * fp32 partial tiles and needs no initialisation.  With it, the output tiles that would form a partly filled last wave
-   * are cut along K and summed in fp32 (fixed order) by the last unit to arrive, and split-K weight gradients are reduced
-   * the same way instead of with bf16 atomics.  NULL: whole tiles / bf16 red.global.add only. */
+   * are cut along K and summed in fp32 (fixed order) by the last unit to arrive.  It serves only that K-split tail: split-K
+   * accumulations (out += A.B, the weight gradients) add each split's partial with bf16 red.global.add whether or not a
+   * workspace is given.  NULL: no K-split tail. */
   void* workspace;
   int64_t workspace_bytes;
 } dvla_gemm_args;
@@ -391,7 +392,7 @@ int dvla_set_sm_budget(int n_sms);
  * Workspace sizes (bytes) of the ops that need caller-provided scratch -- the library never allocates device memory:
  *   attn_bwd : `delta` fp32 [B, H, Lq]  (rowsum(dO * O), FlashAttention-2 backward)
  *   silog    : `stats` fp32 [2]         (sum d, sum d^2; zeroed by the caller before dvla_silog_stats)
- *   gemm     : optional (dvla_gemm_args.workspace): fp32 partial tiles + arrival counters of the K-split tail / split-K
+ *   gemm     : optional (dvla_gemm_args.workspace): fp32 partial tiles + arrival counters of the K-split tail
  * ------------------------------------------------------------------------------------------------------------- */
 int64_t dvla_attn_bwd_workspace_bytes(int64_t B, int64_t H, int64_t Lq);
 int64_t dvla_silog_workspace_bytes(void);

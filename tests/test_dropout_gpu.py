@@ -118,24 +118,6 @@ def test_dropout_kernel_exact(dev, L, case):
 
 
 # ============================================== GEMM epilogue =========================================================
-def gemm_plan(L, a, b, *, out, bias=None, residual=None, act=0, dropout_p=0.0):
-    """dvla_gemm_plan of the call _lib.gemm(a, b, ...) makes (a [M,K], b [N,K], both K-major)."""
-    import ctypes as C
-    args = L.GemmArgs()
-    args.a, args.b, args.out = a.data_ptr(), b.data_ptr(), out.data_ptr()
-    args.bias = None if bias is None else bias.data_ptr()
-    if residual is not None:
-        args.residual, args.ldr = residual.data_ptr(), residual.stride(0)
-    args.M, args.N, args.K = a.shape[0], b.shape[0], a.shape[1]
-    args.lda, args.ldb, args.ldo = a.stride(0), b.stride(0), out.stride(0)
-    args.act, args.alpha, args.dropout_p = act, 1.0, dropout_p
-    ws = L.gemm_workspace(a.device)
-    args.workspace, args.workspace_bytes = ws.data_ptr(), ws.numel()
-    info = L.GemmPlanInfo()
-    assert L.load().dvla_gemm_plan(C.byref(args), C.byref(info)) == 0, L.load().dvla_last_error()
-    return info
-
-
 GEMM_CASES = [  # (id, M, N, K, lda or None, expected kernel, expect a K-split tail)
     ("wgmma", 300, 520, 256, None, 2, False),
     ("wgmma_ksplit_tail", 2580, 1024, 4096, None, 2, True),
@@ -168,7 +150,7 @@ def test_gemm_dropout_epilogue(dev, L, case):
     # 1. the mask alone: positive operands, no bias / act / residual
     a, w = _operands(dev, M, N, K, lda, g, positive=True)
     out = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
-    info = gemm_plan(L, a, w, out=out, dropout_p=p)
+    info = L.gemm_plan(a, w, out=out, dropout_p=p)
     assert info.kernel == kernel, f"{name}: expected GEMM kernel {kernel}, the plan says {info.kernel}"
     assert (info.tail_splits > 1) == tail, f"{name}: tail_splits={info.tail_splits}"
     L.gemm(a, w, out=out, dropout_p=p, dropout_seed=SEED, dropout_seed_ptr=sp)
@@ -179,7 +161,7 @@ def test_gemm_dropout_epilogue(dev, L, case):
     bias = torch.randn(N, generator=g).to(dev, torch.bfloat16)
     res = torch.randn(M, N, generator=g).to(dev, torch.bfloat16)
     out = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
-    info = gemm_plan(L, a, w, out=out, bias=bias, residual=res, act=L.ACT_GELU_TANH, dropout_p=p)
+    info = L.gemm_plan(a, w, out=out, bias=bias, residual=res, act=L.ACT_GELU_TANH, dropout_p=p)
     assert info.kernel == kernel and (info.tail_splits > 1) == tail, (name, info.kernel, info.tail_splits)
     L.gemm(a, w, out=out, bias=bias, act=L.ACT_GELU_TANH, residual=res, dropout_p=p, dropout_seed=SEED, dropout_seed_ptr=sp)
     kt = torch.from_numpy(keep).to(dev)

@@ -7,7 +7,8 @@ Checked over the GEMM shapes of the C2 / C3 / C4 workloads, their weight-gradien
   * a tail starts on a wave boundary, only exists for GEMMs of at least one full wave (batch-invariance of the sub-wave
     GEMMs of action inference, tests/test_rollout_gpu.py), and its partial tiles fit the workspace;
   * without a workspace there is no tail; pure accumulations (out == residual) may split K, everything else may not;
-  * the SM budget (`dvla_set_sm_budget`, lowered while NCCL shares the GPU) resizes grids and moves the wave boundary.
+  * the SM budget (`dvla_set_sm_budget`, lowered while NCCL shares the GPU) resizes grids and moves the wave boundary;
+  * every case of the GPU path table (tests/gemm_cases.py) plans the kernel path it declares, at 132 and 114 SMs.
 """
 import ctypes as C
 import random
@@ -15,6 +16,7 @@ import random
 import pytest
 
 from dreamvla_b200 import _lib, build
+from tests import gemm_cases as GC
 
 FAKE = 0x7F0000000000        # aligned fake device addresses: the planner only tests pointers for NULL / alignment
 
@@ -164,3 +166,54 @@ def test_random_shapes(lib):
         if not accumulate:
             check_tail(lib, p, us, 132)
             assert p.k_splits == 1
+
+
+def plan_case(lib, c):
+    """dvla_gemm_plan of a tests/gemm_cases.py case, with fake pointers offset like the case's matrices."""
+    esz = 4 if c.out_fp32 else 2
+    a = _lib.GemmArgs()
+    a.a, a.b = FAKE + 2 * c.a_off, FAKE + (1 << 32) + 2 * c.b_off
+    a.out = FAKE + (2 << 32) + esz * c.out_off
+    a.M, a.N, a.K = c.M, c.N, c.K
+    a.lda, a.ldb, a.ldo = c.lda, c.ldb, c.ldo
+    a.a_mn_major, a.b_mn_major = int(c.a_mn), int(c.b_mn)
+    a.act, a.out_fp32, a.alpha = c.act, int(c.out_fp32), c.alpha
+    if c.has_bias:
+        a.bias = FAKE + (3 << 32)
+    if c.residual_is_out:
+        a.residual, a.ldr = a.out, c.ldo
+    elif c.has_residual:
+        a.residual, a.ldr = FAKE + (5 << 32) + esz * c.res_off, c.ldr
+    if c.recipe == "full":
+        a.aux_out, a.ld_aux = FAKE + (6 << 32) + 2 * c.aux_off, c.ld_aux
+    elif c.recipe == "dgrad":
+        a.aux_in, a.ld_aux = FAKE + (6 << 32) + 2 * c.aux_off, c.ld_aux
+    if c.recipe == "dropout":
+        a.dropout_p, a.dropout_seed_ptr = GC.DROPOUT_P, FAKE + (7 << 32)
+    a.workspace, a.workspace_bytes = FAKE + (4 << 32), int(lib.dvla_gemm_workspace_bytes(None))
+    out = _lib.GemmPlanInfo()
+    assert lib.dvla_gemm_plan(C.byref(a), C.byref(out)) == 0, lib.dvla_last_error()
+    return out
+
+
+@pytest.mark.parametrize("sms", GC.SM_BUDGETS)
+def test_case_table_paths(lib, sms):
+    """Every case of tests/gemm_cases.py reaches the path it declares, at the SM counts of the H100 SXM and PCIe; and the
+    table covers every path with every reachable majorness x recipe, and every activation on a staged and a direct path."""
+    lib.dvla_set_sm_budget(sms)
+    try:
+        wrong = []
+        for c in GC.CASES:
+            got = GC.path_of(plan_case(lib, c), c)
+            if got != c.path_at(sms):
+                wrong.append(f"{c.id}: plans {got}")
+        assert not wrong, f"{len(wrong)} cases leave their declared path at {sms} SMs:\n" + "\n".join(wrong[:20])
+    finally:
+        lib.dvla_set_sm_budget(0)
+    have = {(c.path, c.a_mn, c.b_mn, c.recipe) for c in GC.CASES}
+    for path in GC.PATHS:
+        recipes = {"wgmma_splitk": ("accum",), "wgmma_tail": ("plain", "full", "dgrad", "dropout")}.get(path, GC.RECIPES)
+        missing = [(path, a, b, r) for (a, b) in GC.MAJORS for r in recipes if (path, a, b, r) not in have]
+        assert not missing, missing
+    acts = {(c.path in GC.STAGED_PATHS, c.act) for c in GC.CASES if c.recipe in ("full", "dgrad", "dropout")}
+    assert all((staged, act) in acts for staged in (True, False) for act in range(6)), sorted(acts)

@@ -1,5 +1,6 @@
-"""GPU parity tests of every kernel behind the C ABI against plain PyTorch fp32 references of the same op
-(tolerances are relative L2 errors of bf16 results vs the fp32 reference; written in tools/gpu_kernel_check.py)."""
+"""GPU parity tests of the normalisation, attention, loss and element-wise kernels behind the C ABI against plain PyTorch
+fp32 references of the same op (tolerances are relative L2 errors of bf16 results vs the fp32 reference; written in
+tools/gpu_kernel_check.py).  The GEMM is checked element by element against fp64 in tests/test_gemm_paths_gpu.py."""
 import os
 import sys
 
@@ -19,7 +20,7 @@ def chk():
     return c
 
 
-@pytest.mark.parametrize("group", ["gemm_basic", "gemm_epilogue", "gemm_splitk", "gemm_tail", "norm", "attn", "loss", "act_bwd_colsum"])
+@pytest.mark.parametrize("group", ["norm", "attn", "loss", "act_bwd_colsum"])
 def test_kernel_group(chk, group):
     chk.RESULTS.clear()
     chk.GROUPS[group]()
